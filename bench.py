@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — SeedVR2-3B upscaled frames/s on B200 (BASELINE.json metric).
+"""bench.py — SeedVR2-3B upscaled frames/s on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N --steps K --warmup W] [--workload 4k_shard|1080p|...] [--impl reference]
 
@@ -13,7 +13,7 @@ the decoded frames.  Output: ONE JSON line on rank 0 (see the task contract).
   value : frames/s, inputs resident in HBM, CUDA-event timed, max over ranks
   e2e   : same through SeedVR2Engine.upscale_clip with pinned HOST input frames
           (H2D inside the timed region) and the result read back to host (D2H)
-  roofline : the tcgen05 GEMM/implicit-conv kernel (dominant): algorithmic FLOPs of
+  roofline : the wgmma GEMM/implicit-conv kernel (dominant): algorithmic FLOPs of
           all its launches / their CUDA-event time, vs the measured bf16 peak
   cpu_baseline : the oracle port (torch fp32, all host threads) on a bounded sample
 """
@@ -39,7 +39,8 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = {
     # name: (real frames, H, W, description)
-    "4k_shard": (8, 2160, 3840, "SeedVR2-3B bf16, 8-frame (->9) 720p->4K clip per GPU = BASELINE config 3 shard"),
+    # 4K shards of 5 frames: the decode of a 9-frame 4K clip needs a 126 GiB workspace, more than an 80 GB H100 holds
+    "4k_shard": (4, 2160, 3840, "SeedVR2-3B bf16, 4-frame (->5) 720p->4K clip per GPU (BASELINE config 3 at 4 instead of 8 frames per GPU)"),
     "1080p": (16, 1080, 1920, "SeedVR2-3B bf16, 16-frame (->17) 540p->1080p clip = BASELINE config 2"),
     "4k_clip64": (64, 2160, 3840, "SeedVR2-3B bf16, 64-frame (->65) 720p->4K as ONE clip on one GPU = BASELINE config 3' "
                                   "(17 latent frames, 2083-token windows, temporally sliced VAE)"),
@@ -200,6 +201,24 @@ def kernel_table(prof, steps, peak_tf, peak_gbs, step_ms):
     return rows
 
 
+DUMP_MAX_VALUES = 8 << 20     # 32 MB of float32
+
+
+def dump_outputs(out_dir, y):
+    """The step's output as float32 .npy: whole when small, else a fixed seeded sample of DUMP_MAX_VALUES values (the
+    same flat indices on every run: torch.randint with seed 1234, sorted) so that two builds can be compared value for value."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    flat = y.detach().reshape(-1)
+    np.save(os.path.join(out_dir, "output_shape.npy"), np.asarray(tuple(y.shape), dtype=np.float64))
+    if flat.numel() <= DUMP_MAX_VALUES:
+        np.save(os.path.join(out_dir, "output.npy"), flat.float().cpu().numpy().reshape(tuple(y.shape)))
+        return
+    g = torch.Generator().manual_seed(1234)
+    idx = torch.randint(0, flat.numel(), (DUMP_MAX_VALUES,), generator=g).sort().values
+    np.save(os.path.join(out_dir, "output_sample.npy"), flat[idx.to(flat.device)].float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -223,6 +242,9 @@ def main():
                          "metric is quoted with 'none' = the north_star path (encode + DiT + decode)")
     ap.add_argument("--phases", action="store_true", help="print a per-kernel breakdown to stderr")
     ap.add_argument("--detail", action="store_true", help="with --phases: break GEMM/conv launches down by shape")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (all ranks' clips with --gpus > 1) as DIR/<name>.npy (float32; a fixed seeded sample of "
+                         "at most 8M values when the output is larger)")
     args = ap.parse_args()
     frames_real, H, W, desc = WORKLOADS[args.workload]
     vae_only = args.workload.startswith("vae_decode")
@@ -260,7 +282,7 @@ def main():
         out_host = torch.empty(frames_real, H, W, 3, dtype=torch.bfloat16).pin_memory()
     frames_dev = frames_host.to(dev)
     gather_buf = torch.empty((world,) + tuple(out_host.shape), device=dev, dtype=torch.bfloat16) if world > 1 else None
-    # a buffer larger than L2 (126 MB) written between steps is unnecessary: every step streams > 10 GB of activations
+    # a buffer larger than L2 (50 MB) written between steps is unnecessary: every step streams > 10 GB of activations
     noise = None
 
     def step(src):
@@ -290,11 +312,18 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record()
+    y_last = None
     for _ in range(args.steps):
-        step(frames_dev)
+        y_last = step(frames_dev)
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and y_last is not None:
+        # what a caller of the timed path receives: the clip, or on N GPUs the all-gathered clips of every rank
+        out = gather_buf if world > 1 else y_last
+        if rank == 0:
+            dump_outputs(args.dump_outputs, out)
+    del y_last
     launches = lib.LAUNCHES
     peak_mem_native = torch.cuda.max_memory_allocated()
     # ---- region P: the same steps with per-kernel CUDA events on the launching stream (per-call events need the Python
@@ -382,9 +411,11 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_gbs = peaks.get("hbm_gbs", 6500.0)
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1.4 PFLOP/s sustained (of fallback)"
+    peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+    peak_gbs = peaks.get("hbm_gbs", 3350.0)
+    peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks
+                else "H100 SXM data sheet: 989 TFLOP/s dense bf16, 3.35 TB/s, at 700 W; a card with a lower power limit "
+                     "reaches less")
     gemm_names = ("svr2_linear_bf16", "svr2_linear_ex_bf16", "svr2_linear_qkv_rope_bf16", "svr2_conv3d_bf16",
                   "svr2_conv3d_stats_bf16", "svr2_conv3d_shortcut_stats_bf16", "svr2_upsample_shuffle_bf16")
     is_gemm = lambda n: n.split("|")[0] in gemm_names
@@ -393,20 +424,6 @@ def main():
     g_calls = sum(d["calls"] for n, d in prof.items() if is_gemm(n))
     achieved = g_flops / (g_ms / 1e3) / 1e12 if g_ms > 0 else 0.0
     fm = flop_model(frames_pad, H, W, variant)
-    # DRAM traffic of the dominant kernel: NOT measured in this run (that needs ncu) — taken from the committed
-    # `ncu --set full` capture of one representative launch and labelled as such; null when the workload does not run it
-    traffic, traffic_detail = None, None
-    try:
-        cap_file = next(f for f in ("ncu_full_r2.json", "ncu_full_r1.json") if os.path.exists(os.path.join(ROOT, "profiles", f)))
-        cap = json.load(open(os.path.join(ROOT, "profiles", cap_file)))["conv256_pair"]
-        if H >= 1080 and not args.workload.startswith("image"):
-            traffic = (float(cap["dram__bytes_read.sum"]) + float(cap["dram__bytes_write.sum"])) * 1e9   # bytes per launch
-            traffic_detail = {"source": f"static: profiles/{cap_file} (ncu --set full of one launch, not this run)",
-                              "algorithmic_bytes_per_launch": (4 + 2) * 1080 * 1920 * 256 * 2.0,
-                              "launch": "conv3d 256->256 3x3x3, 2 frames 1080x1920 (+2 halo frames)",
-                              "tensor_pipe_active_pct": float(cap["sm__mem_tensor_cycles_active.avg.pct_of_peak_sustained_elapsed"])}
-    except Exception:
-        pass
     if args.phases:
         tot = sum(d["ms"] for d in prof.values())
         for n, d in sorted(prof.items(), key=lambda kv: -kv[1]["ms"]):
@@ -446,9 +463,9 @@ def main():
                 "note": ("SeedVR2Engine.vae_decode on a pinned host latent; decoded frames copied back to host" if vae_only else
                          "SeedVR2Engine.upscale_clip on pinned host frames at the source resolution (resized on the device); result copied back to host")},
         "gpu_launches": launches,
-        "roofline": {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (Linear + implicit-GEMM Conv3d + upsample)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_wgmma_kernel (Linear + implicit-GEMM Conv3d + upsample)",
                      "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
-                     "traffic": traffic, "traffic_detail": traffic_detail, "launches": g_calls, "kernel_ms_per_step": g_ms / prof_steps,
+                     "launches": g_calls, "kernel_ms_per_step": g_ms / prof_steps,
                      "share_of_step": g_ms / ms_prof, "profiled_ms_per_step": ms_prof / prof_steps, "peak_source": peak_src,
                      "note": "achieved = algorithmic FLOPs only (a duplicated QK^T pass of the VAE attention counts as time, not work)"},
         "kernels": kernel_table(prof, prof_steps, peak_tf, peak_gbs, ms_prof / prof_steps),

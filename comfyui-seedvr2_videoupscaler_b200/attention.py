@@ -1,6 +1,6 @@
 """The literal ``attention_mode`` seam: a drop-in for the reference's
 ``FlashAttentionVarlen`` (``src/models/dit_3b/attention.py:77-148``) backed by the
-tcgen05 kernel ``svr2_attn_varlen_bf16`` — same call signature, same packed
+wgmma kernel ``svr2_attn_varlen_bf16`` — same call signature, same packed
 (total, heads, 128) layout, same int32 cu_seqlens, returns compute-dtype output.
 
 A maintainer registers it as ``attention_mode="b200"`` (see INTEGRATION.md); unlike

@@ -1,4 +1,4 @@
-"""Builds csrc/libsvr2.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds csrc/libsvr2.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libsvr2.so")
 SOURCES = ["api.cu", "gemm.cu", "attn.cu", "elementwise.cu", "post.cu", "pre.cu", "engine.cu", "vae_engine.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
@@ -39,7 +39,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             print(f"--- {src}\n{out}")
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {src}")
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode:
         print(r.stdout)

@@ -11,7 +11,7 @@ plus ``sample_to_image`` = ``optimized_sample_to_image_format`` + ``clamp(-1,1)*
 (``generation_phases.py:1322-1345``) and ``apply_color_correction`` = the method switch of
 ``generation_phases.py:1299-1317``.  Tensors are ``[T, 3, H, W]`` in ``[-1, 1]`` on the GPU; results are bf16 (the
 pipeline's compute dtype).  Every op is a libsvr2.so kernel (``csrc/post.cu``); there is no torch fallback.
-``hsv`` and ``wavelet_adaptive`` are not part of the B200 path (they raise).
+``hsv`` and ``wavelet_adaptive`` are not part of the engine's path (they raise).
 """
 from __future__ import annotations
 
@@ -129,5 +129,5 @@ def apply_color_correction(sample: torch.Tensor, input_video: torch.Tensor, colo
     if color_correction == "adain":
         return adaptive_instance_normalization(sample, input_video)
     if color_correction in ("hsv", "wavelet_adaptive"):
-        raise NotImplementedError(f"color_correction={color_correction!r} is not part of the B200 path")
+        raise NotImplementedError(f"color_correction={color_correction!r} is not part of the engine's path")
     raise ValueError(f"unknown color_correction {color_correction!r}")

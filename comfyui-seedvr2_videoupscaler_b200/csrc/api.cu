@@ -26,6 +26,6 @@ extern "C" int svr2_device_check(int* sm_count, int* cc_major, int* cc_minor) {
   if (sm_count) *sm_count = prop.multiProcessorCount;
   if (cc_major) *cc_major = prop.major;
   if (cc_minor) *cc_minor = prop.minor;
-  if (prop.major != 10) return svr2::set_error(SVR2_ERR_ARCH, "libsvr2 requires an sm_100 (B200) device");
+  if (prop.major != 9) return svr2::set_error(SVR2_ERR_ARCH, "libsvr2 requires an sm_90 (H100) device");
   return SVR2_OK;
 }

@@ -1,4 +1,4 @@
-// K4 — varlen (windowed) self-attention for head_dim = 128 on tcgen05.
+// K4 — varlen (windowed) self-attention for head_dim = 128 on wgmma (sm_90a).
 //
 // Drop-in for FlashAttentionVarlen.forward / pytorch_varlen_attention
 // (reference dit_3b/attention.py:27-64, 114-148): for every sequence i (one Swin
@@ -6,14 +6,14 @@
 //      O_i = softmax(Q_i K_i^T / sqrt(128)) V_i        (non-causal, no mask)
 // on the packed (total, heads, 128) bf16 layout with int32 cu_seqlens.
 //
-// Persistent CTAs (two per SM) walk the work list (q-tile of 128 rows, head, sequence); 6 warps:
-//   warp 0    : TMA producer  (Q per item, a 2-stage ring of K tiles and a V tile, 128B swizzle; runs ahead into the next item)
-//   warp 1    : MMA issuer    (S = Q K^T: SS-MMA M=128,N=64,K=16; O += P V: TS-MMA with P as the A operand in tensor
-//                              memory, V consumed straight from its row-major tile as an MN-major B operand; fp32 in TMEM)
-//   warps 2-5 : softmax       (one query row per thread: tcgen05.ld the S row, online softmax in registers with exp2
-//                              and a thresholded rescale, P -> bf16 pairs -> tcgen05.st into 32 TMEM columns,
-//                              final 1/l and the scatter store through out_row_map)
-// (PTM = false keeps the earlier path: P through swizzled shared memory + fence.proxy.async, an SS-MMA for P V.)
+// One CTA per work item (q-tile of 128 rows, head, sequence); 9 warps:
+//   warps 0-7 : two consumer warpgroups, 64 query rows each:
+//               S = Q K^T   wgmma m64n64k16, Q and K from 128B-swizzled smem (K-major), fp32 S in registers;
+//               online softmax on the accumulator fragment (row max / sum over the 4 lanes sharing a row, exp2);
+//               O += P V    wgmma m64n128k16 with P as the register A operand (bf16 pairs of the S fragment) and V
+//                           straight from its row-major tile as an MN-major B operand; fp32 O in registers;
+//               final 1/l and the scatter store through out_row_map
+//   warp 8    : TMA producer (Q once, a 2-stage ring of K + V tiles)
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -26,30 +26,22 @@
 
 namespace svr2 {
 
-__device__ __forceinline__ float fast_exp2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 constexpr int ATT_BM = 128;      // q rows per CTA
-constexpr int ATT_BN = 64;       // kv rows per tile (two CTAs are co-resident per SM: ~98 KB smem each)
+constexpr int ATT_BN = 64;       // kv rows per tile
 constexpr int ATT_D = 128;
-constexpr int ATT_THREADS = 192;
+constexpr int ATT_THREADS = 288;
+constexpr int ATT_STAGES = 2;
 constexpr int ATT_Q_BYTES = 128 * 128 * 2;          // 32 KB: two [128 x 64] swizzled halves
 constexpr int ATT_QH_BYTES = ATT_Q_BYTES / 2;
 constexpr int ATT_KV_BYTES = ATT_BN * 128 * 2;      // 16 KB: two [64 x 64] swizzled halves
 constexpr int ATT_KVH_BYTES = ATT_KV_BYTES / 2;
-constexpr int ATT_P_BYTES = 128 * ATT_BN * 2;       // 16 KB: one [128 x 64] swizzled block
 
 struct AttnSmem {
   // offsets inside the 1024-aligned dynamic smem
   static constexpr int kQ = 0;
-  static constexpr int kP = kQ + ATT_Q_BYTES;
-  static constexpr int kK = kP + ATT_P_BYTES;
-  static constexpr int kV = kK + ATT_KV_BYTES;
-  static constexpr int kK1 = kV + ATT_KV_BYTES;      // second K stage
-  static constexpr int kBar = kK1 + ATT_KV_BYTES;
+  static constexpr int kK = kQ + ATT_Q_BYTES;                      // ATT_STAGES K tiles
+  static constexpr int kV = kK + ATT_STAGES * ATT_KV_BYTES;        // ATT_STAGES V tiles
+  static constexpr int kBar = kV + ATT_STAGES * ATT_KV_BYTES;
   static constexpr int kTotal = kBar + 128 + 1024;
 };
 
@@ -60,336 +52,165 @@ struct AttnParams {
   int heads;
   float scale_log2;  // softmax_scale * log2(e)
   int n_qt;          // q tiles per sequence (of the longest sequence)
-  int n_work;        // n_qt * n_seq * heads work items
 };
 
-// Persistent CTAs (two per SM): every CTA walks the work list (q-tile, sequence, head) with a fixed stride, so barrier
-// setup, the TMEM allocation and — above all — the TMA round trip for Q and the first K tiles are paid once per CTA
-// instead of once per 128 query rows: the producer warp runs ahead into the next work item while the softmax warps
-// finish the current one, and the first S = Q K^T of the next item is issued as soon as the score buffer is free.
-// Inside an item the software pipeline is the same as before: S_{j+1} = Q K_{j+1}^T is issued as soon as the softmax
-// warps have pulled S_j into registers, P_j V_j runs while tile j+1 is in its softmax; K is double-buffered, V single.
-// All barrier phases are tracked with running counters (tiles / items processed by this CTA).
-// POLY: three of every eight column pairs of a full tile take their exp2 on the FMA pipe (ptx.cuh exp2_poly, relative
-// error 5e-5 against the 4e-3 of the bf16 rounding that follows): the 64 ex2 per row and tile keep the MUFU pipe busy
-// exactly as long as the tile's two MMAs keep the tensor pipe (512 cycles each), and both of an SM's CTAs share it.
-// PTM: the probabilities go to tensor memory (tcgen05.st, 32 columns of packed bf16 pairs next to S) and P V is a
-// TS-MMA (A operand from TMEM) instead of st.shared + fence.proxy.async + an SS-MMA: the generic->async proxy fence and
-// the arrive behind it were 25 % of the softmax warps' stall samples (profiles/ncu_attn_r2.md); the barrier polls for
-// pv_done / the next s_full are issued early so that their round trip overlaps the exponentials / the P store.
-template <bool POLY, bool PTM>
-__global__ void __launch_bounds__(ATT_THREADS, 2)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_varlen_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                    const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AttnSmem::kBar);
   uint64_t* q_full = bars + 0;
-  uint64_t* k_full = bars + 1;
-  uint64_t* k_empty = bars + 2;
-  uint64_t* v_full = bars + 3;
-  uint64_t* v_empty = bars + 4;
-  uint64_t* s_full = bars + 5;
-  uint64_t* s_free = bars + 6;
-  uint64_t* p_ready = bars + 7;
-  uint64_t* pv_done = bars + 8;
-  uint64_t* k_full1 = bars + 9;                    // second K stage
-  uint64_t* k_empty1 = bars + 10;
-  uint64_t* q_empty = bars + 11;                   // all Q K^T of an item issued and retired: Q may be overwritten
-  uint64_t* o_free = bars + 12;                    // the epilogue has read O: the next item's P V may overwrite it
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
+  uint64_t* kv_full = bars + 1;                    // [ATT_STAGES]
+  uint64_t* kv_empty = bars + 1 + ATT_STAGES;      // [ATT_STAGES]
+
+  // work item -> (q tile, head, sequence); q tiles of one (sequence, head) are neighbours so that the CTAs running
+  // at the same time share its K / V through L2
+  const int w = blockIdx.x;
+  const int qt = w % p.n_qt;
+  const int rest = w / p.n_qt;
+  const int head = rest % p.heads;
+  const int seq = rest / p.heads;
+  const int s_begin = p.cu_seqlens[seq];
+  const int len = p.cu_seqlens[seq + 1] - s_begin;
+  if (qt * ATT_BM >= len) return;                  // uniform over the CTA
+  const int n_kv = (len + ATT_BN - 1) / ATT_BN;
+  const int col0 = head * ATT_D;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    mbar_init(k_full, 1);
-    mbar_init(k_empty, 1);
-    mbar_init(k_full1, 1);
-    mbar_init(k_empty1, 1);
-    mbar_init(v_full, 1);
-    mbar_init(v_empty, 1);
-    mbar_init(s_full, 1);
-    mbar_init(s_free, 128);
-    mbar_init(p_ready, 128);
-    mbar_init(pv_done, 1);
-    mbar_init(q_empty, 1);
-    mbar_init(o_free, 128);
+    for (int s = 0; s < ATT_STAGES; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], 2);                  // one arrive per consumer warpgroup
+    }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<256>(tmem_slot);     // S: 64 columns, O: 128 columns
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_s = tmem_base, tmem_p = tmem_base + 64, tmem_o = tmem_base + 128;
 
-  // work item w -> (q tile, head, sequence); q tiles of one (sequence, head) are neighbours so that the CTAs running
-  // at the same time share its K / V through L2
-  const int n_qt = p.n_qt, n_work = p.n_work;
-  auto decode = [&](int w, int& qt, int& head, int& s_begin, int& len) {
-    qt = w % n_qt;
-    const int rest = w / n_qt;
-    head = rest % p.heads;
-    const int seq = rest / p.heads;
-    s_begin = p.cu_seqlens[seq];
-    len = p.cu_seqlens[seq + 1] - s_begin;
-  };
-
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
-      uint32_t it = 0, kq = 0, vq = 0;             // items, K tiles, V tiles loaded so far
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-        int qt, head, s_begin, len;
-        decode(w, qt, head, s_begin, len);
-        if (qt * ATT_BM >= len) continue;
-        const int n_kv = (len + ATT_BN - 1) / ATT_BN;
-        const int col0 = head * ATT_D, q_row0 = s_begin + qt * ATT_BM;
-        mbar_wait(q_empty, (it & 1) ^ 1);
-        mbar_expect_tx(q_full, ATT_Q_BYTES);
-        tma_load_2d(smem + AttnSmem::kQ, &tmap_q, q_full, col0, q_row0);
-        tma_load_2d(smem + AttnSmem::kQ + ATT_QH_BYTES, &tmap_q, q_full, col0 + 64, q_row0);
-        auto load_k = [&](int j) {                 // K_j -> stage kq & 1 (its previous tenant was the K tile two loads ago)
-          const int st = kq & 1;
-          uint64_t* full = st ? k_full1 : k_full;
-          uint64_t* empty = st ? k_empty1 : k_empty;
-          uint8_t* dst = smem + (st ? AttnSmem::kK1 : AttnSmem::kK);
-          const int r0 = s_begin + j * ATT_BN;
-          mbar_wait(empty, ((kq >> 1) & 1) ^ 1);
-          mbar_expect_tx(full, ATT_KV_BYTES);
-          tma_load_2d(dst, &tmap_k, full, col0, r0);
-          tma_load_2d(dst + ATT_KVH_BYTES, &tmap_k, full, col0 + 64, r0);
-          ++kq;
-        };
-        load_k(0);
-        if (n_kv > 1) load_k(1);
-        for (int j = 0; j < n_kv; ++j) {
-          const int r0 = s_begin + j * ATT_BN;
-          mbar_wait(v_empty, (vq & 1) ^ 1);
-          mbar_expect_tx(v_full, ATT_KV_BYTES);
-          tma_load_2d(smem + AttnSmem::kV, &tmap_v, v_full, col0, r0);
-          tma_load_2d(smem + AttnSmem::kV + ATT_KVH_BYTES, &tmap_v, v_full, col0 + 64, r0);
-          ++vq;
-          if (j + 2 < n_kv) load_k(j + 2);         // waits for Q K_j^T to retire
-        }
-        ++it;
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+      const int q_row0 = s_begin + qt * ATT_BM;
+      mbar_expect_tx(q_full, ATT_Q_BYTES);
+      tma_load_2d(smem + AttnSmem::kQ, &tmap_q, q_full, col0, q_row0);
+      tma_load_2d(smem + AttnSmem::kQ + ATT_QH_BYTES, &tmap_q, q_full, col0 + 64, q_row0);
+      for (int j = 0; j < n_kv; ++j) {
+        const int s = j % ATT_STAGES;
+        const int r0 = s_begin + j * ATT_BN;
+        mbar_wait(&kv_empty[s], ((j / ATT_STAGES) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[s], 2 * ATT_KV_BYTES);
+        uint8_t* k_dst = smem + AttnSmem::kK + s * ATT_KV_BYTES;
+        uint8_t* v_dst = smem + AttnSmem::kV + s * ATT_KV_BYTES;
+        tma_load_2d(k_dst, &tmap_k, &kv_full[s], col0, r0);
+        tma_load_2d(k_dst + ATT_KVH_BYTES, &tmap_k, &kv_full[s], col0 + 64, r0);
+        tma_load_2d(v_dst, &tmap_v, &kv_full[s], col0, r0);
+        tma_load_2d(v_dst + ATT_KVH_BYTES, &tmap_v, &kv_full[s], col0 + 64, r0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = umma_idesc_bf16(128, ATT_BN, 0, 0);
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(128, 128, 0, 1);  // B (=V) is MN-major
-      const uint32_t q_addr = smem_u32(smem + AttnSmem::kQ);
-      const uint32_t p_addr = smem_u32(smem + AttnSmem::kP);
-      const uint32_t k_addr = smem_u32(smem + AttnSmem::kK);
-      const uint32_t v_addr = smem_u32(smem + AttnSmem::kV);
-      uint32_t it = 0, kc = 0, g = 0;              // items, K tiles consumed, S tiles produced (== tiles started)
-      uint32_t gp = 0;                             // P V products issued
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-        int qt, head, s_begin, len;
-        decode(w, qt, head, s_begin, len);
-        if (qt * ATT_BM >= len) continue;
-        const int n_kv = (len + ATT_BN - 1) / ATT_BN;
-        auto issue_qk = [&](bool last) {           // next S = Q K^T into the (single) score buffer
-          if (g > 0) mbar_wait(s_free, (g - 1) & 1);       // the softmax warps hold the previous S in registers
-          const int st = kc & 1;
-          mbar_wait(st ? k_full1 : k_full, (kc >> 1) & 1);
-          tc_fence_after();
-          const uint32_t kb = st ? smem_u32(smem + AttnSmem::kK1) : k_addr;
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {                 // contraction over d = 128
-            const uint64_t da = umma_desc_kmajor_sw128(q_addr + (kk >> 2) * ATT_QH_BYTES) + uint64_t((kk & 3) * 2);
-            const uint64_t db = umma_desc_kmajor_sw128(kb + (kk >> 2) * ATT_KVH_BYTES) + uint64_t((kk & 3) * 2);
-            umma_bf16(tmem_s, da, db, idesc_qk, kk != 0);
-          }
-          umma_commit(st ? k_empty1 : k_empty);            // this K stage may be refilled
-          if (last) umma_commit(q_empty);                  // and Q, by the next item
-          umma_commit(s_full);
-          ++kc;
-          ++g;
-        };
-        mbar_wait(q_full, it & 1);
-        issue_qk(n_kv == 1);
-        for (int j = 0; j < n_kv; ++j) {
-          if (j + 1 < n_kv) issue_qk(j + 2 == n_kv);       // next scores while tile j is in its softmax
-          mbar_wait(v_full, gp & 1);
-          mbar_wait(p_ready, gp & 1);                      // P_j in smem, O rescaled
-          if (j == 0) mbar_wait(o_free, (it & 1) ^ 1);     // the previous item's O has been read out
-          tc_fence_after();
-#pragma unroll
-          for (int kk = 0; kk < ATT_BN / 16; ++kk) {       // contraction over the 64 kv rows (16 per MMA)
-            const uint64_t db = umma_desc_mnmajor_sw128(v_addr + kk * 16 * 128, ATT_KVH_BYTES, 1024);
-            if constexpr (PTM) {
-              umma_bf16_ts(tmem_o, tmem_p + kk * 8, db, idesc_pv, (j | kk) != 0);
-            } else {
-              const uint64_t da = umma_desc_kmajor_sw128(p_addr) + uint64_t(kk * 2);
-              umma_bf16(tmem_o, da, db, idesc_pv, (j | kk) != 0);
-            }
-          }
-          umma_commit(v_empty);
-          umma_commit(pv_done);
-          ++gp;
-        }
-        ++it;
-      }
-    }
-  } else {
-    // ------------------------------ softmax warps (2..5)
-    const int quad = warp & 3;                 // TMEM lane quadrant accessible to this warp
-    const int row = quad * 32 + lane;          // query row within the tile
-    const uint32_t lane_off = uint32_t(quad * 32) << 16;
-    // m_ref is the row maximum the exponentials are taken against.  It only moves when the running maximum has grown
-    // by more than 2^kGrow since (FA4's thresholded rescale): P then holds values up to 2^kGrow instead of <= 1 — exact
-    // in fp32 / bf16 (relative rounding), and the O rescale below (four TMEM round trips on the critical path) becomes
-    // rare instead of happening on almost every early tile.
-    constexpr float kGrow = 8.0f;
-    const float sc = p.scale_log2;
-    const uint32_t sp_row = smem_u32(smem + AttnSmem::kP) + row * 128;
-    uint32_t g = 0;                            // tiles processed by this CTA (phase of s_full / s_free / p_ready / pv_done)
-    for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-      int qt, head, s_begin, len;
-      decode(w, qt, head, s_begin, len);
-      if (qt * ATT_BM >= len) continue;
-      const int n_kv = (len + ATT_BN - 1) / ATT_BN;
-      float m_ref = -INFINITY, l_run = 0.f;
-      bool s_ok = false;                          // PTM: s_full of this tile already seen complete by the early poll
-      for (int j = 0; j < n_kv; ++j, ++g) {
-        if (!(PTM && s_ok)) mbar_wait(s_full, g & 1);
-        tc_fence_after();
-        uint32_t sv[ATT_BN];
-        tmem_ld32(tmem_s + lane_off + 0, *reinterpret_cast<uint32_t(*)[32]>(&sv[0]));
-        tmem_ld32(tmem_s + lane_off + 32, *reinterpret_cast<uint32_t(*)[32]>(&sv[32]));
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(s_free);                      // S may be overwritten by the next QK^T
-        const int kv_valid = len - j * ATT_BN;    // columns >= kv_valid are padding / the next sequence
-        const bool ragged = kv_valid < ATT_BN;
-        if (ragged) {                             // only the last tile of a sequence is ragged
-#pragma unroll
-          for (int c = 0; c < ATT_BN; ++c)
-            if (c >= kv_valid) sv[c] = 0xff800000u;   // -inf
-        }
-        // row maximum: four independent chains of 3-input max
-        float mx4[4];
-#pragma unroll
-        for (int a = 0; a < 4; ++a) mx4[a] = __uint_as_float(sv[a]);
-#pragma unroll
-        for (int c = 4; c < ATT_BN; c += 8) {
-#pragma unroll
-          for (int a = 0; a < 4; ++a)
-            mx4[a] = fmaxf(fmaxf(mx4[a], __uint_as_float(sv[c + a])), __uint_as_float(sv[(c + 4 + a) & (ATT_BN - 1)]));
-        }
-        const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-        bool pv_ok = false;
-        if constexpr (PTM) {
-          if (j > 0) pv_ok = mbar_try_wait(pv_done, (g - 1) & 1);     // round trip hidden behind the exponentials
-        }
-        const bool grow = (mx - m_ref) * sc > kGrow;                   // true on the first tile (m_ref = -inf)
-        const float m_new = grow ? mx : m_ref;
-        const float alpha = grow ? fast_exp2((m_ref - m_new) * sc) : 1.0f;   // 0 on the first tile
-        const float2 nmb = make_float2(-m_new * sc, -m_new * sc);
-        const float2 sc2 = make_float2(sc, sc);
-        // P = exp2(s * sc - m_new * sc): packed fp32x2 FMAs, four independent partial sums
-        float2 ls[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-        uint32_t pk[ATT_BN / 2];
-        if (POLY && !ragged) {                    // (a masked -inf would come out of the polynomial as 2^-125, not 0)
-#pragma unroll
-          for (int c = 0; c < ATT_BN; c += 2) {
-            const float2 t = ffma2(make_float2(__uint_as_float(sv[c]), __uint_as_float(sv[c + 1])), sc2, nmb);
-            const int i8 = (c >> 1) & 7;
-            const bool poly = i8 == 1 || i8 == 4 || i8 == 6;          // folds after unrolling
-            const float2 e = poly ? make_float2(exp2_poly(t.x), exp2_poly(t.y)) : make_float2(fast_exp2(t.x), fast_exp2(t.y));
-            ls[(c >> 1) & 1] = fadd2(ls[(c >> 1) & 1], e);
-            pk[c / 2] = pack_bf16x2(e.x, e.y);
-          }
-        } else {
-#pragma unroll
-          for (int c = 0; c < ATT_BN; c += 2) {
-            const float2 t = ffma2(make_float2(__uint_as_float(sv[c]), __uint_as_float(sv[c + 1])), sc2, nmb);
-            const float2 e = make_float2(fast_exp2(t.x), fast_exp2(t.y));
-            ls[(c >> 1) & 1] = fadd2(ls[(c >> 1) & 1], e);
-            pk[c / 2] = pack_bf16x2(e.x, e.y);
-          }
-        }
-        const float lsum = (ls[0].x + ls[1].x) + (ls[0].y + ls[1].y);
-        if (j > 0) {
-          if (!(PTM && pv_ok)) mbar_wait(pv_done, (g - 1) & 1);   // P_{j-1} V_{j-1} has read the P buffer and updated O
-          tc_fence_after();
-          if (__any_sync(0xffffffffu, grow)) {
-#pragma unroll 1
-            for (int c0 = 0; c0 < 128; c0 += 64) {
-              uint32_t o[64];
-              tmem_ld32(tmem_o + lane_off + c0, *reinterpret_cast<uint32_t(*)[32]>(&o[0]));
-              tmem_ld32(tmem_o + lane_off + c0 + 32, *reinterpret_cast<uint32_t(*)[32]>(&o[32]));
-              tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < 64; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-              tmem_st32(tmem_o + lane_off + c0, *reinterpret_cast<const uint32_t(*)[32]>(&o[0]));
-              tmem_st32(tmem_o + lane_off + c0 + 32, *reinterpret_cast<const uint32_t(*)[32]>(&o[32]));
-            }
-            tmem_st_wait();
-          }
-        }
-        if constexpr (PTM) {
-          // P -> tensor memory: this thread's row, 32 columns of packed pairs (keys 2c, 2c + 1 in column c)
-          tmem_st32(tmem_p + lane_off, *reinterpret_cast<const uint32_t(*)[32]>(&pk[0]));
-          l_run = l_run * alpha + lsum;
-          m_ref = m_new;
-          s_ok = (j + 1 < n_kv) && mbar_try_wait(s_full, (g + 1) & 1);   // next scores: poll behind the store's wait
-          tmem_st_wait();
-          tc_fence_before();
-          mbar_arrive(p_ready);
-        } else {
-          // P -> swizzled K-major smem (row = this thread, 8 chunks of 16 B); explicit shared-space stores
-#pragma unroll
-          for (int ch = 0; ch < ATT_BN / 8; ++ch)
-            st_shared_v4(sp_row + ((ch ^ (row & 7)) << 4), pk[4 * ch], pk[4 * ch + 1], pk[4 * ch + 2], pk[4 * ch + 3]);
-          l_run = l_run * alpha + lsum;
-          m_ref = m_new;
-          fence_proxy_async_smem();                  // make P visible to the tensor core (async proxy)
-          tc_fence_before();
-          mbar_arrive(p_ready);
-        }
-      }
-      // ------------------------------ epilogue: O / l -> bf16 -> global
-      mbar_wait(pv_done, (g - 1) & 1);
-      tc_fence_after();
-      const float inv_l = 1.0f / l_run;
-      const int q_idx = qt * ATT_BM + row;
-      const bool valid = q_idx < len;
-      long long grow_ = (long long)(s_begin + q_idx);
-      if (valid && p.out_row_map) grow_ = p.out_row_map[grow_];
-      __nv_bfloat16* orow = p.out + (grow_ * p.heads + head) * ATT_D;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 64) {
-        uint32_t o[64];
-        tmem_ld32(tmem_o + lane_off + c0, *reinterpret_cast<uint32_t(*)[32]>(&o[0]));
-        tmem_ld32(tmem_o + lane_off + c0 + 32, *reinterpret_cast<uint32_t(*)[32]>(&o[32]));
-        tmem_ld_wait();
-        if (c0 == 64) {                            // all of O is in registers: the next item may start accumulating
-          tc_fence_before();
-          mbar_arrive(o_free);
-        }
-        if (valid) {
-#pragma unroll
-          for (int e = 0; e < 64; e += 8) {
-            uint4 pk4 = make_uint4(pack_bf16x2(__uint_as_float(o[e]) * inv_l, __uint_as_float(o[e + 1]) * inv_l),
-                                   pack_bf16x2(__uint_as_float(o[e + 2]) * inv_l, __uint_as_float(o[e + 3]) * inv_l),
-                                   pack_bf16x2(__uint_as_float(o[e + 4]) * inv_l, __uint_as_float(o[e + 5]) * inv_l),
-                                   pack_bf16x2(__uint_as_float(o[e + 6]) * inv_l, __uint_as_float(o[e + 7]) * inv_l));
-            *reinterpret_cast<uint4*>(orow + c0 + e) = pk4;
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
+
+  // ------------------------------ consumer warpgroups
+  const int wg = warp >> 2;                        // rows [64 wg, 64 wg + 64) of the q tile
+  const int quad = lane & 3;
+  const int r_lo = wg * 64 + ((warp & 3) << 4) + (lane >> 2);   // this thread's rows: r_lo and r_lo + 8
+  const float sc = p.scale_log2;
+  const uint32_t q_addr = smem_u32(smem + AttnSmem::kQ) + wg * 64 * 128;
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int s = j % ATT_STAGES;
+    mbar_wait(&kv_full[s], (j / ATT_STAGES) & 1);
+    const uint32_t k_addr = smem_u32(smem + AttnSmem::kK + s * ATT_KV_BYTES);
+    const uint32_t v_addr = smem_u32(smem + AttnSmem::kV + s * ATT_KV_BYTES);
+    float sv[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {                 // contraction over d = 128
+      const uint64_t da = wgmma_desc_kmajor_sw128(q_addr + (kk >> 2) * ATT_QH_BYTES) + uint64_t((kk & 3) * 2);
+      const uint64_t db = wgmma_desc_kmajor_sw128(k_addr + (kk >> 2) * ATT_KVH_BYTES) + uint64_t((kk & 3) * 2);
+      wgmma_ss<ATT_BN>(sv, da, db, kk != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sv);
+
+    const int kv_valid = len - j * ATT_BN;           // columns >= kv_valid are padding / the next sequence
+    if (kv_valid < ATT_BN) {                         // only the last tile of a sequence is ragged
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if ((i >> 2) * 8 + 2 * quad + (i & 1) >= kv_valid) sv[i] = -INFINITY;
+    }
+    // row maxima (fragment rows: even register pairs -> r_lo, odd pairs -> r_lo + 8), reduced over the 4 lanes of a row
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 32; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sv[i]);
+    float alpha[2], nmb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m_run[h], mx[h]);
+      alpha[h] = exp2_approx((m_run[h] - m_new) * sc);  // 0 on the first tile (m_run = -inf)
+      nmb[h] = -m_new * sc;
+      m_run[h] = m_new;
+    }
+    // P = exp2(s * sc - m * sc): fp32 row sums, bf16 pairs packed in the A-operand fragment order
+    float ls[2] = {0.f, 0.f};
+    uint32_t pa[16];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float e0 = exp2_approx(fmaf(sv[i], sc, nmb[h]));
+      const float e1 = exp2_approx(fmaf(sv[i + 1], sc, nmb[h]));
+      ls[h] += e0 + e1;
+      pa[i >> 1] = pack_bf16x2(e0, e1);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + ls[h];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+
+    wgmma_fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < ATT_BN / 16; ++kk) {       // contraction over the 64 kv rows (16 per MMA)
+      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+      const uint64_t db = wgmma_desc_mnmajor_sw128(v_addr + kk * 16 * 128, ATT_KVH_BYTES, 1024);
+      wgmma_rs_tb<ATT_D>(o, a, db, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[s]);   // K_j / V_j fully read by this warpgroup
+  }
+
+  // ------------------------------ epilogue: O / l -> bf16 -> global
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float inv_l = 1.0f / l_run[h];
+    const int q_idx = qt * ATT_BM + r_lo + 8 * h;
+    if (q_idx >= len) continue;
+    long long grow_ = (long long)(s_begin + q_idx);
+    if (p.out_row_map) grow_ = p.out_row_map[grow_];
+    __nv_bfloat16* orow = p.out + (grow_ * p.heads + head) * ATT_D;
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+      const int i = 4 * c + 2 * h;
+      *reinterpret_cast<uint32_t*>(orow + 8 * c + 2 * quad) = pack_bf16x2(o[i] * inv_l, o[i + 1] * inv_l);
+    }
   }
 }
 
@@ -403,17 +224,7 @@ extern "C" int svr2_attn_varlen_bf16(const void* q, const void* k, const void* v
   if (n_seq <= 0 || total <= 0) return SVR2_OK;
   if (max_seqlen <= 0) return set_error(SVR2_ERR_ARG, "svr2_attn_varlen_bf16: max_seqlen must be > 0");
   static bool configured[64] = {};                // the attribute is per (function, device)
-  // A/B switches: SVR2_ATTN_POLY=1 part of the exp2 on the FMA pipe (measured slower: 0.878 vs 0.842 ms on 243 x 463 x 20);
-  // SVR2_ATTN_PTMEM=0 the probabilities through shared memory (the round-1 / early round-2 path)
-  static int poly = -1, ptm = -1;
-  if (poly < 0) {
-    const char* e = getenv("SVR2_ATTN_POLY");
-    poly = e ? atoi(e) : 0;
-    const char* t = getenv("SVR2_ATTN_PTMEM");
-    ptm = t ? atoi(t) : 1;
-  }
-  auto kern = ptm ? (poly ? attn_varlen_kernel<true, true> : attn_varlen_kernel<false, true>)
-                  : (poly ? attn_varlen_kernel<true, false> : attn_varlen_kernel<false, false>);
+  auto kern = attn_varlen_kernel;
   const int dev = current_device();
   if (!configured[dev]) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
@@ -439,8 +250,6 @@ extern "C" int svr2_attn_varlen_bf16(const void* q, const void* k, const void* v
   p.n_qt = (max_seqlen + ATT_BM - 1) / ATT_BM;
   const long long n_work = (long long)p.n_qt * n_seq * heads;
   if (n_work > 0x7fffffffLL) return set_error(SVR2_ERR_ARG, "svr2_attn_varlen_bf16: too many work items");
-  p.n_work = (int)n_work;
-  const int grid = (int)(n_work < 2LL * num_sms() ? n_work : 2LL * num_sms());   // persistent: two CTAs per SM
-  kern<<<grid, ATT_THREADS, AttnSmem::kTotal, (cudaStream_t)stream>>>(tq, tk, tv, p);
+  kern<<<(unsigned)n_work, ATT_THREADS, AttnSmem::kTotal, (cudaStream_t)stream>>>(tq, tk, tv, p);
   return check_launch("attn_varlen");
 }

@@ -1034,7 +1034,7 @@ int svr2::ncdhw_to_ndhwc_strided(const void* in, int in_dtype, int C, int T, int
                                  int C_pad, int out_t_pad, float div, void* stream) {
   const long long total = (long long)T * H * W;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   cudaStream_t s = (cudaStream_t)stream;
   const long long cs = chan_stride;
   if (in_dtype == 0) ncdhw_to_ndhwc_kernel<float><<<blocks, 256, 0, s>>>((const float*)in, C, T, H, W, cs, (__nv_bfloat16*)out, C_pad, out_t_pad, div);
@@ -1051,7 +1051,7 @@ int svr2::ndhwc_to_ncdhw_strided(const void* in, int ld_in, int C, int T, int H,
                                  int64_t chan_stride, void* stream) {
   const long long total = (long long)T * H * W;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   cudaStream_t s = (cudaStream_t)stream;
   const long long cs = chan_stride;
   if (out_dtype == 0) ndhwc_to_ncdhw_kernel<float><<<blocks, 256, 0, s>>>((const __nv_bfloat16*)in, ld_in, C, T, H, W, (float*)out, cs);
@@ -1073,7 +1073,7 @@ extern "C" int svr2_im2col3_bf16(const void* x, int T, int H, int W, int C, int 
   }
   const long long total = (long long)T * H * W * (ld_out / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 64) blocks = 148LL * 64;
+  if (blocks > 132LL * 64) blocks = 132LL * 64;
   im2col3_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, T, H, W, C, ld_in, (__nv_bfloat16*)out, ld_out);
   return check_launch("im2col3");
 }
@@ -1085,7 +1085,7 @@ int svr2::conv_tap_gather_strided(const float* z, int64_t ldz, int co_n, const v
   if (co_n < 1 || co_n > 4) return set_error(SVR2_ERR_ARG, "conv_tap_gather: 1 <= co_n <= 4");
   const long long total = (long long)T * H * W;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   cudaStream_t s = (cudaStream_t)stream;
   const long long cs = chan_stride;
   if (out_dtype == 0)

@@ -1,6 +1,6 @@
-// K1/K6 — persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// K1/K6 — persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   D[M,N] = A[M,K] · B[N,K]^T   (bf16 x bf16 -> fp32 in TMEM -> fused epilogue)
+//   D[M,N] = A[M,K] · B[N,K]^T   (bf16 x bf16 -> fp32 in registers -> fused epilogue)
 //
 // One kernel body serves the DiT Linear layers (A = activation rows, 2-D TMA)
 // and the VAE causal Conv3d as an implicit GEMM (A = shifted NDHWC boxes fetched
@@ -9,10 +9,10 @@
 //
 // Roles (384 threads, 1 CTA / SM, grid = #SMs, static tile schedule):
 //   warps 0,3 : TMA producers (even / odd k-blocks of a kStages-deep smem ring, 128B-swizzled K-major tiles)
-//   warp 1 : MMA issuer     (one elected lane, tcgen05.mma cta_group::1, M=128,N=BLOCK_N,K=16)
-//   warp 2 : TMEM allocator (2 accumulator stages so the epilogue overlaps the next tile)
-//   warps 4-11: epilogue    (tcgen05.ld 32x32b -> registers -> fused math -> swizzled smem slab ->
-//                            row-contiguous 16-byte global stores; two warps per TMEM lane quadrant)
+//   warps 1,2 : idle
+//   warps 4-11: two MMA warpgroups (wgmma m64 x BLOCK_N x 16, 64 tile rows each, fp32 accumulators in registers),
+//               then the epilogue (accumulators -> fp32 tile in shared memory over the drained ring -> one row per
+//               thread -> fused math -> swizzled smem slab -> row-contiguous 16-byte global stores)
 //
 // Reference semantics replaced: nn.Linear (dit_3b/mmattn.py:56-59,173,269; mlp.py:56-61;
 // patch_v1.py:37,62), InflatedCausalConv3d (causal_inflation_lib.py:213-305), Upsample3D's
@@ -35,8 +35,8 @@ namespace svr2 {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
-constexpr int UMMA_K = 16;
-constexpr int kNumThreads = 384;   // 4 control warps + 8 epilogue warps
+constexpr int WGMMA_K = 16;
+constexpr int kNumThreads = 384;   // 4 producer-side warps + 2 MMA / epilogue warpgroups
 
 struct GemmParams {
   int M, N, K;
@@ -102,10 +102,10 @@ enum : int {
   EPI_ROWSCALE = 1024,  // acc *= rowscale[m] first (un-normalised probabilities x V, divided by the row sum)
 };
 
-template <int BLOCK_N, bool TWO = false>
+template <int BLOCK_N>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
-  static constexpr int kBBytes = (TWO ? BLOCK_N / 2 : BLOCK_N) * BLOCK_K * 2;   // a CTA pair splits B along N
+  static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStagingBytes = 8 * 4096;            // epilogue: 8 warps x (32 rows x 128 B)
   static constexpr int kBudget = 232448 - kStagingBytes - 256 - 1024;   // 227 KB max dynamic smem
@@ -114,6 +114,17 @@ struct SmemLayout {
   static constexpr int kBarOffset = kStagingOffset + kStagingBytes;
   static constexpr int kTotal = kBarOffset + 256 + 1024;  // barriers + alignment slack
 };
+
+// 32 consecutive fp32 accumulator columns of one row of the shared accumulator tile (idx: element offset, % 4 == 0)
+__device__ __forceinline__ void acc_ld32(const float* acc, uint32_t idx, uint32_t (&v)[32]) {
+  const float4* s = reinterpret_cast<const float4*>(acc + idx);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 t = s[i];
+    v[4 * i] = __float_as_uint(t.x); v[4 * i + 1] = __float_as_uint(t.y);
+    v[4 * i + 2] = __float_as_uint(t.z); v[4 * i + 3] = __float_as_uint(t.w);
+  }
+}
 
 // per-lane GroupNorm partial sums of the 8 bf16 values a lane stores (channels 0-3 -> x/y, 4-7 -> z/w)
 __device__ __forceinline__ void stat_acc(float4& a, const uint4& d) {
@@ -131,10 +142,6 @@ __device__ __forceinline__ void stat_acc(float4& a, const uint4& d) {
 // ordered band-major: a band of `band_h` tile rows is swept over ALL output frames before the next band, so the
 // three temporal taps (and the vertical 3x3 halo inside the band) hit L2.
 __device__ __forceinline__ void conv_tile(const GemmParams& p, int m_blk, int& t_o, int& th, int& tw) {
-  if (m_blk >= p.num_m_tiles) {   // odd tile count in pair mode: the phantom tile reads out-of-bounds (zero) frames
-    t_o = p.T_out; th = 0; tw = 0;
-    return;
-  }
   const int full = p.T_out * p.band_h * p.tiles_w;          // m-tiles in a full band
   const int band = m_blk / full;
   const int r = m_blk - band * full;
@@ -149,7 +156,7 @@ __device__ __forceinline__ void conv_tile(const GemmParams& p, int m_blk, int& t
 }
 
 // L2-aware tile raster: the n-tiles are processed in groups of `g` columns of tiles; inside a group the order is
-// m-major with n fastest, so a group's slice of B (g * BLOCK_N * K * 2 bytes, chosen <= ~24 MB by the host) stays
+// m-major with n fastest, so a group's slice of B (g * BLOCK_N * K * 2 bytes, chosen <= ~16 MB by the host) stays
 // L2-resident while A streams through once per group.  (Plain n-fastest order re-streams all of B from DRAM for
 // every m-row once B exceeds L2 — 132 MB for the 4K VAE attention keys.)
 __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int g, int& m, int& n) {
@@ -217,46 +224,26 @@ __device__ __forceinline__ RowDest row_dest(const GemmParams& p, int epi, int m_
 
 // SWAP (conv only, BLOCK_N = 256): operands exchanged so that M = 128 output channels (weights as A)
 // and N = 256 output pixels (activation box as B).  Cout = 128 layers then run 128x256 tiles instead of
-// 128x128 ones, whose SS-MMA shared-memory read rate (128 B/clk) caps them near 1 PFLOP/s.
-// TWO: a cluster of 2 CTAs (one SM pair) works on a 256 x BLOCK_N tile with tcgen05.mma.cta_group::2:
-// each CTA loads its own 128 A rows and half of the B rows, CTA 0 issues the MMAs for both, each CTA
-// drains its own 128 x BLOCK_N accumulator.  Halves the B traffic per SM and the per-SM smem read rate.
+// 128x128 ones (half the weight traffic per output, twice the MMA work per k-block).
 // EPI_CT >= 0: the epilogue flags are a compile-time constant (p.epi must equal it) — the per-element loops then carry
 // no runtime flag tests.  A single such test cost the short-K pixel-shuffle GEMM 50 % (its epilogue, ~1 800 warp
 // instructions per tile, is the whole kernel); EPI_CT = -1 keeps the generic runtime-flag epilogue.
-// WR (CTA pairs, stride-1 3x3-spatial convs only): W-reuse mainloop — an m-tile is ONE output row segment of 128 pixels per
-// CTA, so the three horizontal taps of a (kt, kh, 64-channel block) read the same 130-pixel input row segment: it is loaded
-// once (boxes of 128 + 8 pixels into a 17 KB stage) and the taps' MMAs address it through A descriptors whose start is
-// shifted by kw rows of 128 B (see conv_wreuse_kernel).  Activation traffic per SM drops 3x: 21.7 KB instead of 32 KB of
-// operands per k-block — these kernels run at 97 % tensor-pipe activity but power-capped far below the boost clock, and
-// L2 -> SM operand traffic is a large part of that power.  Two rings: kWrNA activation stages, kWrNB weight k-blocks.
-constexpr int kWrNA = 4, kWrNB = 7, kWrABytes = 136 * 128;
-template <int BLOCK_N, int KIND, bool SWAP = false, bool TWO = false, int EPI_CT = -1, bool WR = false>
+template <int BLOCK_N, int KIND, bool SWAP = false, int EPI_CT = -1>
 __global__ void __launch_bounds__(kNumThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                    const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_a_tail,
-                    const GemmParams p) {
-  static_assert(!(SWAP && TWO), "swap-AB and CTA pairs are mutually exclusive");
-  static_assert(!WR || (TWO && BLOCK_N == 256 && KIND == KIND_BF16), "the W-reuse mainloop exists for the CTA-pair bf16 conv kernel");
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_a2, const GemmParams p) {
   if (p.run_if != nullptr && *p.run_if == 0) return;     // conditional launch: every thread of every CTA sees the same flag
-  using L = SmemLayout<BLOCK_N, TWO>;
-  const uint32_t cta_rank = TWO ? cluster_ctarank() : 0u;
+  using L = SmemLayout<BLOCK_N>;
   constexpr int kStages = L::kStages;
-  constexpr int ACC_STRIDE = BLOCK_N < 32 ? 32 : BLOCK_N;   // TMEM columns per accumulator stage
-  constexpr uint32_t kTmemCols = (2 * ACC_STRIDE <= 64) ? 64 : (2 * ACC_STRIDE <= 128) ? 128
-                                 : (2 * ACC_STRIDE <= 256) ? 256 : 512;
+  constexpr int ACC_STRIDE = BLOCK_N < 32 ? 32 : BLOCK_N;   // accumulator columns the epilogue addresses
+  constexpr int ACC_LD = ACC_STRIDE + 4;                    // fp32 row pitch of the shared accumulator tile
+  static_assert(BLOCK_M * ACC_LD * 4 <= L::kStagingOffset, "the accumulator tile overlays the operand ring");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
   uint64_t* empty_bar = full_bar + kStages;
-  // WR: full_bar = [activation stages | weight stages], empty_bar likewise
-  constexpr int kBars = WR ? kWrNA + kWrNB : kStages;
-  if constexpr (WR) empty_bar = full_bar + kBars;
-  static_assert(!WR || (kWrNA * kWrABytes + kWrNB * (BLOCK_N / 2) * BLOCK_K * 2 <= L::kStagingOffset && 2 * kBars + 5 <= 32),
-                "W-reuse rings must fit the generic kernel's operand region and barrier block");
-  uint64_t* tmem_full = empty_bar + kBars;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* acc_free = empty_bar + kStages;      // the epilogue is done with the accumulator tile (it overlays the ring)
+  const float* acc_s = reinterpret_cast<const float*>(smem);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -267,176 +254,32 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     if (p.extra_blocks) tma_prefetch_desc(&tmap_a2);
   }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < kBars; ++i) {
+    for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);                  // one arrive per consumer warpgroup
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], TWO ? 512 : 256);   // pair: the epilogue threads of both CTAs arrive at CTA 0
-    }
+    mbar_init(acc_free, 256);
     fence_barrier_init();
   }
-  if constexpr (TWO) cluster_sync_all();            // barriers of both CTAs initialised before any remote arrive
-  if (warp == 2) {
-    if constexpr (TWO) tmem_alloc_2cta<kTmemCols>(tmem_slot);
-    else tmem_alloc<kTmemCols>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // tile schedule: 1-CTA: one 128-row m-tile per tile; pair: m-tiles (2j, 2j+1) per tile, same tile in both CTAs
   const int num_n_tiles = p.num_n_tiles;
-  const int num_m_sup = TWO ? (p.num_m_tiles + 1) / 2 : p.num_m_tiles;
-  const int num_tiles = num_m_sup * num_n_tiles;
-  const int tile0 = TWO ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = TWO ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int num_m_tiles = p.num_m_tiles;
+  const int num_tiles = num_m_tiles * num_n_tiles;
+  const int tile0 = (int)blockIdx.x;
+  const int tile_step = (int)gridDim.x;
 
-  // W-reuse schedule shared by the three roles: (kt, kh, cb) groups of three k-blocks (kw = 0, 1, 2), the fused shortcut's
-  // single-k-block stages spread evenly between them (see conv_wreuse_kernel)
-  const int wr_groups = p.taps_t * 3 * p.cin_blocks;
-  auto wr_extras_after = [&](int gi, int e) {
-    if (e >= p.extra_blocks) return false;
-    const int pos = (e + 1) * wr_groups / (p.extra_blocks + 1);
-    return (pos < 1 ? 1 : pos) == gi + 1;
-  };
-  if (WR && warp == 0) {
-    // ------------------------- W-reuse: activation row segments, one stage per (kt, kh, cb) + one per shortcut block
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      auto acquire = [&](uint32_t bytes) -> uint8_t* {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], 2 * bytes);         // both CTAs' bytes land on CTA 0's barrier
-        return smem + stage * kWrABytes;
-      };
-      auto advance = [&]() { if (++stage == kWrNA) { stage = 0; phase ^= 1; } };
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        int m_sup, n_blk;
-        tile_coords(tile, num_m_sup, num_n_tiles, p.group_n, m_sup, n_blk);
-        int t_o, th, tw;
-        conv_tile(p, 2 * m_sup + (int)cta_rank, t_o, th, tw);
-        const int w0 = tw * 128;
-        int gi = 0, e = 0;
-        for (int kt_ = 0; kt_ < p.taps_t; ++kt_) {
-          const int t_in = t_o * p.stride_t + kt_;
-          for (int kh_ = 0; kh_ < 3; ++kh_) {
-            const int h_in = th + kh_ - 1;
-            for (int cb = 0; cb < p.cin_blocks; ++cb, ++gi) {
-              uint8_t* sa = acquire(kWrABytes);
-              tma2_load_4d(sa, &tmap_a, &full_bar[stage], cb * BLOCK_K, w0 - 1, h_in, t_in);
-              tma2_load_4d(sa + 128 * 128, &tmap_a_tail, &full_bar[stage], cb * BLOCK_K, w0 + 127, h_in, t_in);
-              advance();
-              for (; wr_extras_after(gi, e); ++e) {      // fused 1x1x1 shortcut: the block input at the output pixels
-                uint8_t* sx = acquire(128 * 128);
-                tma2_load_4d(sx, &tmap_a2, &full_bar[stage], e * BLOCK_K, w0, th, t_o);
-                advance();
-              }
-            }
-          }
-        }
-      }
-    }
-  } else if (WR && (warp == 3 || warp == 2)) {
-    // ------------------------- W-reuse: this CTA's half of the weight rows, one stage per k-block, in MMA order.  Two
-    // threads (warp 3: even k-blocks, warp 2 — the TMEM allocator, idle in the main loop — odd ones): one producer
-    // iteration (barrier poll, expect-tx, TMA issue) costs ~500 cycles, the k-block's MMAs 512
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t turn = warp == 3 ? 0u : 1u;
-      constexpr int kWBytes = (BLOCK_N / 2) * BLOCK_K * 2;
-      uint8_t* wbase = smem + kWrNA * kWrABytes;
-      const int cin = p.cin;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        int m_sup, n_blk;
-        tile_coords(tile, num_m_sup, num_n_tiles, p.group_n, m_sup, n_blk);
-        const int n0 = n_blk * BLOCK_N + (int)cta_rank * (BLOCK_N / 2);
-        auto load = [&](int kcol) {
-          if ((turn++ & 1u) == 0u) {
-            mbar_wait(&empty_bar[kWrNA + stage], phase ^ 1);
-            if (cta_rank == 0) mbar_expect_tx(&full_bar[kWrNA + stage], 2 * kWBytes);
-            tma2_load_2d(wbase + stage * kWBytes, &tmap_b, &full_bar[kWrNA + stage], kcol, n0);
-          }
-          if (++stage == kWrNB) { stage = 0; phase ^= 1; }
-        };
-        int gi = 0, e = 0;
-        for (int g = 0; g < p.taps_t * 3; ++g)            // g = kt * 3 + kh
-          for (int cb = 0; cb < p.cin_blocks; ++cb, ++gi) {
-            for (int kw_ = 0; kw_ < 3; ++kw_) load((g * 3 + kw_) * cin + cb * BLOCK_K);
-            for (; wr_extras_after(gi, e); ++e) load(p.taps_t * 9 * cin + e * BLOCK_K);
-          }
-      }
-    }
-  } else if (WR && warp == 1) {
-    // ------------------------- W-reuse: MMA issuer (CTA 0 of the pair)
-    if (lane == 0 && cta_rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(2 * BLOCK_M, BLOCK_N);
-      constexpr int kWBytes = (BLOCK_N / 2) * BLOCK_K * 2;
-      const uint32_t w_addr0 = smem_u32(smem + kWrNA * kWrABytes);
-      int as = 0, bs = 0, acc = 0;
-      uint32_t aph = 0, bph = 0, acc_phase = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * ACC_STRIDE;
-        // The issuing thread is the critical resource (its per-k-block path — barrier poll, descriptor set-up, four
-        // UTCHMMA with their uniform-register moves, commit — measured 613 cycles against 512 of MMA work in the first
-        // version of this loop): constant-trip tap loop, descriptors advanced by additions, the shortcut schedule
-        // reduced to one comparison per group.
-        uint32_t first = 1;
-        int e = 0;
-        auto next_extra_pos = [&](int e_) {
-          if (e_ >= p.extra_blocks) return 0x7fffffff;
-          const int pos = (e_ + 1) * wr_groups / (p.extra_blocks + 1);
-          return pos < 1 ? 1 : pos;
-        };
-        int extra_pos = next_extra_pos(0);
-        auto taps = [&](const int n_taps) {
-          mbar_wait(&full_bar[as], aph);
-          const uint64_t a_desc0 = umma_desc_kmajor_sw128(smem_u32(smem + as * kWrABytes));
-#pragma unroll
-          for (int kw_ = 0; kw_ < 3; ++kw_) {
-            if (kw_ < n_taps) {
-              mbar_wait(&full_bar[kWrNA + bs], bph);
-              tc_fence_after();
-              const uint64_t a_desc = a_desc0 + uint64_t(kw_ * 8);      // kw rows of 128 B into the stage (address-based swizzle)
-              const uint64_t b_desc = umma_desc_kmajor_sw128(w_addr0 + bs * kWBytes);
-#pragma unroll
-              for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                umma_bf16_2cta(d_tmem, a_desc + uint64_t(k * 2), b_desc + uint64_t(k * 2), idesc, first ? 0u : 1u);
-                first = 0;
-              }
-              umma_commit_2cta(&empty_bar[kWrNA + bs]);
-              if (++bs == kWrNB) { bs = 0; bph ^= 1; }
-            }
-          }
-          umma_commit_2cta(&empty_bar[as]);
-          if (++as == kWrNA) { as = 0; aph ^= 1; }
-        };
-        for (int gi = 0; gi < wr_groups; ++gi) {
-          taps(3);
-          while (extra_pos == gi + 1) {      // the shortcut blocks scheduled after this group
-            taps(1);
-            extra_pos = next_extra_pos(++e);
-          }
-        }
-        umma_commit_2cta(&tmem_full[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp == 0 || warp == 3) {
+  if (warp == 0 || warp == 3) {
     // ========================= TMA producers (2 warps) =========================
-    // One thread of warp 0 feeds the even k-blocks of the ring, one thread of warp 3 the odd ones.
-    // A single producer thread costs ~500 issue cycles per k-block (measured) against 512 cycles of
-    // MMA work per 128x256x64 block, so one producer alone caps the kernel; the per-k-block path is
-    // also kept free of divisions and parameter reloads.
+    // One thread of warp 0 feeds the even k-blocks of the ring, one thread of warp 3 the odd ones, so that the
+    // per-k-block issue path (barrier poll, expect-tx, two TMA issues) of one thread never paces the MMAs.
+    // The shared accumulator tile of the epilogue overlays the ring: a tile's loads start once the previous
+    // tile's epilogue has released it (acc_free).
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       uint32_t g = (warp == 0) ? 0u : 1u;   // parity toggle: handle a k-block when (g & 1) == 0
+      uint32_t it = 0;                      // tiles started by this CTA
       const int a_mode = p.a_mode;
       const int nkb = p.num_k_blocks;
       auto acquire = [&](uint8_t*& sa, uint64_t*& fb) -> bool {
@@ -445,33 +288,28 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
           mbar_wait(&empty_bar[stage], phase ^ 1);
           sa = smem + stage * L::kStageBytes;
           fb = &full_bar[stage];
-          if constexpr (TWO) {
-            if (cta_rank == 0) mbar_expect_tx(fb, 2 * L::kStageBytes);   // bytes of both CTAs land on CTA 0's barrier
-          } else {
-            mbar_expect_tx(fb, L::kStageBytes);
-          }
+          mbar_expect_tx(fb, L::kStageBytes);
         }
         return mine;
       };
       auto advance = [&]() {
         if (++stage == kStages) { stage = 0; phase ^= 1; }
       };
+      auto tile_start = [&]() {
+        if (it > 0) mbar_wait(acc_free, (it - 1) & 1u);
+        ++it;
+      };
       if (a_mode == 0) {
         for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-          int m_sup, n_blk;
-          tile_coords(tile, num_m_sup, num_n_tiles, p.group_n, m_sup, n_blk);
-          const int m_blk = TWO ? 2 * m_sup + (int)cta_rank : m_sup;
-          const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N + (TWO ? (int)cta_rank * (BLOCK_N / 2) : 0);
+          int m_blk, n_blk;
+          tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
+          tile_start();
+          const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
           for (int kb = 0; kb < nkb; ++kb) {
             uint8_t* sa; uint64_t* fb;
             if (acquire(sa, fb)) {
-              if constexpr (TWO) {
-                tma2_load_2d(sa, &tmap_a, fb, kb * BLOCK_K, m0);
-                tma2_load_2d(sa + L::kABytes, &tmap_b, fb, kb * BLOCK_K, n0);
-              } else {
-                tma_load_2d(sa, &tmap_a, fb, kb * BLOCK_K, m0);
-                tma_load_2d(sa + L::kABytes, &tmap_b, fb, kb * BLOCK_K, n0);
-              }
+              tma_load_2d(sa, &tmap_a, fb, kb * BLOCK_K, m0);
+              tma_load_2d(sa + L::kABytes, &tmap_b, fb, kb * BLOCK_K, n0);
             }
             advance();
           }
@@ -480,13 +318,13 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         const int bw = p.bw, bh = p.bh, pad_h = p.pad_h, pad_w = p.pad_w, stride_t = p.stride_t;
         const int taps_t = p.taps_t, taps_h = p.taps_h, taps_w = p.taps_w, cin_blocks = p.cin_blocks, cin = p.cin;
         for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-          int m_sup, n_blk;
-          tile_coords(tile, num_m_sup, num_n_tiles, p.group_n, m_sup, n_blk);
-          const int m_blk = TWO ? 2 * m_sup + (int)cta_rank : m_sup;
+          int m_blk, n_blk;
+          tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
+          tile_start();
           int t_o, th, tw;
           conv_tile(p, m_blk, t_o, th, tw);
           const int h0 = th * bh, w0 = tw * bw;
-          const int n0 = n_blk * (SWAP ? BLOCK_M : BLOCK_N) + (TWO ? (int)cta_rank * (BLOCK_N / 2) : 0);
+          const int n0 = n_blk * (SWAP ? BLOCK_M : BLOCK_N);
           int kcol = 0;
           for (int kt_ = 0; kt_ < taps_t; ++kt_) {
             const int t_in = t_o * stride_t + kt_;
@@ -497,24 +335,14 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
                   if (acquire(sa, fb)) {
                     uint8_t* s_act = SWAP ? sa + L::kABytes : sa;      // activation box
                     uint8_t* s_wgt = SWAP ? sa : sa + L::kABytes;      // weight rows
-                    if constexpr (TWO) {
-                      if (a_mode == 1) {
-                        tma2_load_4d(s_act, &tmap_a, fb, cb * BLOCK_K, w0 + kw_ - pad_w, h0 + kh_ - pad_h, t_in);
-                      } else {
-                        tma2_load_5d(s_act, &tmap_a, fb, (kw_ & 1) * cin + cb * BLOCK_K, w0 + (kw_ >> 1), kh_ & 1,
-                                     h0 + (kh_ >> 1), t_in);
-                      }
-                      tma2_load_2d(s_wgt, &tmap_b, fb, kcol, n0);
+                    if (a_mode == 1) {
+                      tma_load_4d(s_act, &tmap_a, fb, cb * BLOCK_K, w0 + kw_ - pad_w, h0 + kh_ - pad_h, t_in);
                     } else {
-                      if (a_mode == 1) {
-                        tma_load_4d(s_act, &tmap_a, fb, cb * BLOCK_K, w0 + kw_ - pad_w, h0 + kh_ - pad_h, t_in);
-                      } else {
-                        // pair view (2C, W/2, 2, H/2, T): input pixel 2*o + k -> pair o + k/2, phase k%2
-                        tma_load_5d(s_act, &tmap_a, fb, (kw_ & 1) * cin + cb * BLOCK_K, w0 + (kw_ >> 1), kh_ & 1,
-                                    h0 + (kh_ >> 1), t_in);
-                      }
-                      tma_load_2d(s_wgt, &tmap_b, fb, kcol, n0);
+                      // pair view (2C, W/2, 2, H/2, T): input pixel 2*o + k -> pair o + k/2, phase k%2
+                      tma_load_5d(s_act, &tmap_a, fb, (kw_ & 1) * cin + cb * BLOCK_K, w0 + (kw_ >> 1), kh_ & 1,
+                                  h0 + (kh_ >> 1), t_in);
                     }
+                    tma_load_2d(s_wgt, &tmap_b, fb, kcol, n0);
                   }
                   kcol += BLOCK_K;
                   advance();
@@ -528,13 +356,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             if (acquire(sa, fb)) {
               uint8_t* s_act = SWAP ? sa + L::kABytes : sa;
               uint8_t* s_wgt = SWAP ? sa : sa + L::kABytes;
-              if constexpr (TWO) {
-                tma2_load_4d(s_act, &tmap_a2, fb, cb * BLOCK_K, w0, h0, t_o);
-                tma2_load_2d(s_wgt, &tmap_b, fb, kcol, n0);
-              } else {
-                tma_load_4d(s_act, &tmap_a2, fb, cb * BLOCK_K, w0, h0, t_o);
-                tma_load_2d(s_wgt, &tmap_b, fb, kcol, n0);
-              }
+              tma_load_4d(s_act, &tmap_a2, fb, cb * BLOCK_K, w0, h0, t_o);
+              tma_load_2d(s_wgt, &tmap_b, fb, kcol, n0);
             }
             kcol += BLOCK_K;
             advance();
@@ -542,48 +365,61 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    // ========================= MMA issuer =========================
-    if (lane == 0 && cta_rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(TWO ? 2 * BLOCK_M : BLOCK_M, BLOCK_N);
-      const int nkb = p.num_k_blocks;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * ACC_STRIDE;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
-          const uint64_t a_desc = umma_desc_kmajor_sw128(a_addr);
-          const uint64_t b_desc = umma_desc_kmajor_sw128(a_addr + L::kABytes);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            // advance 16 elements (32 B) along K inside the 128-B swizzle row: +2 in the >>4 address field
-            if constexpr (TWO) umma_bf16_2cta(d_tmem, a_desc + uint64_t(k * 2), b_desc + uint64_t(k * 2), idesc, (kb | k) != 0);
-            else umma_bf16(d_tmem, a_desc + uint64_t(k * 2), b_desc + uint64_t(k * 2), idesc, (kb | k) != 0);
-          }
-          // frees the smem slot (in both CTAs of a pair) once the MMAs have read it
-          if constexpr (TWO) umma_commit_2cta(&empty_bar[stage]); else umma_commit(&empty_bar[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        if constexpr (TWO) umma_commit_2cta(&tmem_full[acc]); else umma_commit(&tmem_full[acc]);   // accumulator complete
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else if (warp >= 4) {
-    // ========================= epilogue (8 warps) =========================
-    // Two warps per TMEM lane quadrant (warp % 4), each owning half of the tile's columns, so every
-    // SM sub-partition has two epilogue warps to hide instruction latency.
-    // Phase 1: a thread owns one accumulator row: tcgen05.ld 32 columns at a time, fused math, result
+    // ========================= MMA + epilogue (2 warpgroups) =========================
+    // Mainloop: warpgroup wg owns tile rows [64 wg, 64 wg + 64): one wgmma m64 x BLOCK_N x 16 per 16 columns of K,
+    // fp32 accumulators in registers, A and B straight from the 128B-swizzled stages.  The stage of k-block kb is
+    // released once the MMAs of kb + 1 are issued and those of kb have retired (one MMA group in flight).
+    // The accumulators then go to a row-major fp32 tile in shared memory (over the drained operand ring), and the
+    // epilogue below reads its rows from there:
+    // Two warps per 32-row quadrant (warp % 4), each owning half of the tile's columns.
+    // Phase 1: a thread owns one accumulator row: 32 columns at a time, fused math, result
     //          (bf16 or fp32) into a per-warp XOR-swizzled staging slab (32 rows x 128 B).
     // Phase 2: the warp re-reads the slab row-major so that every global load/store instruction covers
     //          contiguous 128-byte row segments (16 B per lane); residual loads are issued in batches
     //          before use, then add + store (+ halo copies).
+    const int wg = (warp - 4) >> 2;
+    int mstage = 0;
+    uint32_t mphase = 0;
+    uint32_t it = 0;
+    auto mainloop = [&]() {
+      float d[BLOCK_N / 2];
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
+      const int nkb = p.num_k_blocks;
+      const bool leader = (threadIdx.x & 127) == 0;
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full_bar[mstage], mphase);
+        const uint32_t a_addr = smem_u32(smem + mstage * L::kStageBytes);
+        const uint64_t a_desc = wgmma_desc_kmajor_sw128(a_addr + wg * 64 * 128);
+        const uint64_t b_desc = wgmma_desc_kmajor_sw128(a_addr + L::kABytes);
+        wgmma_fence_regs(d);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
+          wgmma_ss<BLOCK_N>(d, a_desc + uint64_t(k * 2), b_desc + uint64_t(k * 2), (kb | k) != 0);
+        wgmma_commit();
+        wgmma_fence_regs(d);
+        wgmma_wait<1>();
+        if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = mstage;
+        if (++mstage == kStages) { mstage = 0; mphase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+      named_bar_sync(1, 256);                    // both warpgroups' MMAs have read their last operands
+      float* acc_w = reinterpret_cast<float*>(smem);
+      const int r0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; i += 4) {
+        const int col = (i >> 2) * 8 + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(acc_w + r0 * ACC_LD + col) = make_float2(d[i], d[i + 1]);
+        *reinterpret_cast<float2*>(acc_w + (r0 + 8) * ACC_LD + col) = make_float2(d[i + 2], d[i + 3]);
+      }
+      named_bar_sync(1, 256);
+    };
     constexpr bool IS_BF16 = KIND == KIND_BF16 || KIND == KIND_BF16_RS;
     constexpr bool IS_PEXP = KIND == KIND_PEXP || KIND == KIND_PEXP_STAT;
     constexpr int N_COLS = KIND == KIND_SWIGLU ? ACC_STRIDE / 2 : ACC_STRIDE;   // output columns per tile
@@ -593,10 +429,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     constexpr int ROWS_PER_IT = 32 / CPR;
     constexpr int N_IT = 32 / ROWS_PER_IT;                                // warp-wide accesses per phase
     constexpr int kBatch = N_IT < 4 ? N_IT : 4;
-    auto tmem_empty_arrive = [&](uint64_t* bar) {
-      if constexpr (TWO) mbar_arrive_cta0(bar); else mbar_arrive(bar);
-    };
-    const int q = warp & 3;               // TMEM lane quadrant this warp may access
+    const int q = warp & 3;               // 32-row quadrant of the tile this warp's epilogue covers
     const int half = (warp - 4) >> 2;     // which half of the columns
     const int row = q * 32 + lane;        // tile row owned by this thread
     const bool active = (N_COLS >= 64) || (half == 0);
@@ -607,12 +440,14 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     const __nv_bfloat16* __restrict__ bias = p.bias;
     const float* __restrict__ gate = p.gate;
     const __nv_bfloat16* __restrict__ resid = p.residual;
-    int acc = 0;
-    uint32_t acc_phase = 0;
     for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-      int m_sup, n_blk;
-      tile_coords(tile, num_m_sup, num_n_tiles, p.group_n, m_sup, n_blk);
-      const int m_blk = TWO ? 2 * m_sup + (int)cta_rank : m_sup;
+      int m_blk, n_blk;
+      tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
+      if (it++ > 0) {                        // the previous tile's epilogue is done with the accumulator tile
+        fence_proxy_async_smem();
+        mbar_arrive(acc_free);
+      }
+      mainloop();
       if constexpr (SWAP) {
         // accumulator lanes = output channels (this thread: co), columns = the tile's 256 pixels.
         int t_o, th, tw;
@@ -623,20 +458,13 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         const float bsc = ((epi & EPI_BIAS) && co < p.N) ? __bfloat162float(bias[co]) : 0.f;
         const long long fbase = (long long)(t_o + p.out_t_pad) * p.out_frame_stride + n_blk * BLOCK_M + q * 32;
         const bool dup_t = p.out_dup_head && t_o == 0;
-        mbar_wait_backoff(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t t_addr = tmem_base + (uint32_t(q * 32) << 16) + acc * ACC_STRIDE;
+        const uint32_t t_addr = row * ACC_LD;
         unsigned short* slab16 = reinterpret_cast<unsigned short*>(slab);
         float4 st = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 1
         for (int c0 = half * 128; c0 < half * 128 + 128; c0 += 32) {
           uint32_t v[32];
-          tmem_ld32(t_addr + c0, v);
-          tmem_ld_wait();
-          if (c0 + 32 >= half * 128 + 128) {
-            tc_fence_before();
-            tmem_empty_arrive(&tmem_empty[acc]);
-          }
+          acc_ld32(acc_s, t_addr + c0, v);
           // transpose through the slab: row = pixel (128 B stride), 32 channels (64 B) per row
 #pragma unroll
           for (int j = 0; j < 32; ++j)
@@ -692,15 +520,13 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
               p.stat_partial[((long long)t_o * p.stat_slots + r * 2 + half) * (p.N / 8) + octet] = st;
           }
         }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         continue;
       }
       RowDest dst = row_dest<BLOCK_N>(p, epi, m_blk, n_blk, row, N_COLS);
-      if (TWO && m_blk >= p.num_m_tiles) { dst.valid = 0; dst.dup = 0; }
       const int n_base = n_blk * (KIND == KIND_SWIGLU ? BLOCK_N / 2 : BLOCK_N);   // first output column
 
       // Wide path (64-column phases): per-column operands live in lane registers (lane l holds columns 2l, 2l+1
-      // of the phase) and are broadcast by shuffle in phase 1; they are fetched before the accumulator wait so
+      // of the phase) and are broadcast by shuffle in phase 1; they are fetched before the accumulator tile is read so
       // the global-load latency never sits on the epilogue's critical path.
       constexpr bool kWide = (IS_BF16 || IS_PEXP) && PH_COLS == 64;
       constexpr int N_PH = kWide ? COLS_W / 64 : 1;
@@ -716,9 +542,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         }
       }
 
-      mbar_wait_backoff(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (uint32_t(q * 32) << 16) + acc * ACC_STRIDE;
+      const uint32_t t_addr = row * ACC_LD;
 
       float row_lse = 0.f;
       float2 st_a = make_float2(0.f, 0.f), st_b = make_float2(0.f, 0.f);   // KIND_PEXP_STAT: this thread's row sum
@@ -741,22 +565,19 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         const int tpw = p.qkv_inner / 256;               // n-tiles per q / k / v
         const int which = n_blk / tpw;                   // 0 q, 1 k, 2 v
         const int m = m_blk * BLOCK_M + row;
-        const bool rvalid = (m < p.M) && !(TWO && m_blk >= p.num_m_tiles);
+        const bool rvalid = (m < p.M);
         uint32_t pk[64];
 #pragma unroll
         for (int c0 = 0; c0 < 128; c0 += 64) {
           uint32_t v0[32], v1[32];
-          tmem_ld32(t_addr + col_lo + c0, v0);
-          tmem_ld32(t_addr + col_lo + c0 + 32, v1);
-          tmem_ld_wait();
+          acc_ld32(acc_s, t_addr + col_lo + c0, v0);
+          acc_ld32(acc_s, t_addr + col_lo + c0 + 32, v1);
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
             pk[c0 / 2 + i] = pack_bf16x2(__uint_as_float(v0[2 * i]), __uint_as_float(v0[2 * i + 1]));
             pk[c0 / 2 + 16 + i] = pack_bf16x2(__uint_as_float(v1[2 * i]), __uint_as_float(v1[2 * i + 1]));
           }
         }
-        tc_fence_before();
-        tmem_empty_arrive(&tmem_empty[acc]);
         if (which < 2) {
           float ss = 0.f;
 #pragma unroll
@@ -821,9 +642,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 #pragma unroll 1
           for (int c0 = col_lo; c0 < col_lo + COLS_W; c0 += RS) {
             uint32_t v[RS];
-            tmem_ld32(t_addr + c0, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-            if constexpr (RS == 64) tmem_ld32(t_addr + c0 + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-            tmem_ld_wait();
+            acc_ld32(acc_s, t_addr + c0, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
+            if constexpr (RS == 64) acc_ld32(acc_s, t_addr + c0 + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
             const int n0 = n_base + c0;
             if (sc > 0.f && n0 + RS <= p.N) {
               // interior step: max on the raw accumulators, the scale folded into the exponent's FMA
@@ -858,32 +678,22 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             }
           }
         }
-        tc_fence_before();
-        tmem_empty_arrive(&tmem_empty[acc]);
         const int m = m_blk * BLOCK_M + row;
         if (active && m < p.M) {
           const int slot = (N_COLS >= 64) ? n_blk * 2 + half : n_blk;
           reinterpret_cast<float2*>(p.out)[(long long)m * p.ldc + slot] = make_float2(mx, sum);
         }
-      } else if (!active) {
-        tc_fence_before();
-        tmem_empty_arrive(&tmem_empty[acc]);
-      } else {
+      } else if (active) {
 #pragma unroll 1
         for (int ph0 = col_lo; ph0 < col_lo + COLS_W; ph0 += PH_COLS) {
           // ---------------- phase 1 ----------------
           if constexpr (kWide) {
-            // both 32-column TMEM chunks of the phase in flight at once; every bf16 rounding point is one
+            // both 32-column accumulator chunks of the phase loaded at once; every bf16 rounding point is one
             // cvt.rn.bf16x2 on a column pair (identical to bf16_rne, half the instructions), and the packed
             // pair is what gets staged
             uint32_t v0[32], v1[32];
-            tmem_ld32(t_addr + ph0, v0);
-            tmem_ld32(t_addr + ph0 + 32, v1);
-            tmem_ld_wait();
-            if (ph0 + PH_COLS >= col_lo + COLS_W) {   // all TMEM reads of this warp are done for this tile
-              tc_fence_before();
-              tmem_empty_arrive(&tmem_empty[acc]);
-            }
+            acc_ld32(acc_s, t_addr + ph0, v0);
+            acc_ld32(acc_s, t_addr + ph0 + 32, v1);
             const int phi = (ph0 - col_lo) / 64;
             uint32_t pk[32];
             const float sc = p.out_scale;
@@ -950,12 +760,11 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 #pragma unroll 1
           for (int c0 = ph0; c0 < ph0 + PH_COLS; c0 += 32) {
             uint32_t v[32];
-            tmem_ld32(t_addr + c0, v);
+            acc_ld32(acc_s, t_addr + c0, v);
             const int n0 = n_base + c0;
             if constexpr (KIND == KIND_SWIGLU) {
               uint32_t u[32];
-              tmem_ld32(t_addr + ACC_STRIDE / 2 + c0, u);
-              tmem_ld_wait();
+              acc_ld32(acc_s, t_addr + ACC_STRIDE / 2 + c0, u);
               // rounding points of the reference's bf16 flow (gate, in, silu(gate), product), one
               // cvt.rn.bf16x2 per column pair each; v[0..15] end up holding the packed output pairs
 #pragma unroll
@@ -968,18 +777,15 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
                                    __uint_as_float(rs & 0xffff0000u) * __uint_as_float(ru & 0xffff0000u));
               }
             } else if constexpr (KIND == KIND_F32) {
-              tmem_ld_wait();
               const float sc = p.out_scale;
 #pragma unroll
               for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * sc);
             } else if constexpr (IS_PEXP) {
-              tmem_ld_wait();
               const float sc = p.out_scale;
 #pragma unroll
               for (int j = 0; j < 32; ++j)
                 v[j] = __float_as_uint(bf16_rne(exp2_approx(__uint_as_float(v[j]) * sc - row_lse)));
             } else {
-              tmem_ld_wait();
               // per-column operands, 8 columns at a time (N % 8 == 0: a group is all-valid or all-OOB)
 #pragma unroll
               for (int g8 = 0; g8 < 4; ++g8) {
@@ -1043,10 +849,6 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
                                __byte_perm(v[8 * j + 4], v[8 * j + 5], 0x7632), __byte_perm(v[8 * j + 6], v[8 * j + 7], 0x7632));
               }
             }
-          }
-          if (ph0 + PH_COLS >= col_lo + COLS_W) {   // all TMEM reads of this warp are done for this tile
-            tc_fence_before();
-            tmem_empty_arrive(&tmem_empty[acc]);
           }
           }   // !kWide
           __syncwarp();
@@ -1121,25 +923,16 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         if constexpr (KIND == KIND_PEXP_STAT) {
           if (p.stat2) {     // this thread's row over this warp's columns of the tile: (max score, sum of exponentials)
             const int m = m_blk * BLOCK_M + row;
-            if (m < p.M && !(TWO && m_blk >= p.num_m_tiles)) {
+            if (m < p.M) {
               const int slot = (N_COLS >= 64) ? n_blk * 2 + half : n_blk;
               p.stat2[(long long)m * p.ld_stat + slot] = make_float2(0.f, (st_a.x + st_b.x) + (st_a.y + st_b.y));
             }
           }
         }
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (TWO) cluster_sync_all();     // the peer may still be arriving on / reading from this CTA
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (TWO) tmem_dealloc_2cta<kTmemCols>(tmem_base);
-    else tmem_dealloc<kTmemCols>(tmem_base);
-  }
 }
 
 // ----------------------------------------------------------------------------
@@ -1202,297 +995,17 @@ int num_sms() {
   return g_num_sms[dev];
 }
 
-// ======================================================================================================================
-// W-reuse conv kernel (Cout <= 128, stride 1, 3x3 spatial taps; swap-AB: M = 128 output channels, N = 256 output pixels).
-//
-// The generic swap-AB kernel moves 48 KB of operands L2 -> SM per 128x256x64 k-block (16 KB of weights + a 32 KB
-// activation box per tap): 96 B/clk and SM, ~13 TB/s chip-wide at 1.2 PFLOP/s — the L2 slices' throughput ceiling, which
-// is what holds those layers at 87 % tensor-pipe activity.  Here a tile is ONE output row segment of 256 pixels, so the
-// three horizontal taps of a (kt, kh, 64-channel block) read the SAME 258-pixel input row segment: it is loaded once
-// (two TMA boxes: 256 + 8 pixels, 128B-swizzled rows) and the three MMAs of the kw taps address it through UMMA
-// descriptors whose start address is shifted by kw rows of 128 B.  Activation traffic drops 3x (27 KB instead of 48 KB
-// per k-block).  Two rings: NB activation stages (33 KB, three k-blocks each) fed by warp 0, NA weight stages (16 KB,
-// one k-block each) fed by warp 3; warp 1 issues, warp 2 owns TMEM, warps 4-11 run the swap-AB epilogue (bias,
-// residual, halo duplication, GroupNorm partial sums) of the generic kernel.
-template <int NB, int NA>
-struct WrSmem {
-  static constexpr int kNB = NB, kNA = NA;
-  static constexpr int kBRows = 264;                       // 256 + 2 halo pixels, rounded to whole 8-row swizzle atoms
-  static constexpr int kBBytes = kBRows * 128;             // 33 792
-  static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;    // 16 384
-  static constexpr int kAOffset = kNB * kBBytes;
-  static constexpr int kStagingOffset = kAOffset + kNA * kABytes;
-  static constexpr int kStagingBytes = 8 * 4096;
-  static constexpr int kBarOffset = kStagingOffset + kStagingBytes;
-  static constexpr int kTotal = kBarOffset + 256 + 1024;
-};
-template <int NB, int NA>
-__global__ void __launch_bounds__(kNumThreads, 1)
-conv_wreuse_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_x_tail,
-                   const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x2,
-                   const GemmParams p) {
-  using L = WrSmem<NB, NA>;
-  static_assert(L::kTotal <= 232448, "W-reuse conv: shared memory budget");
-  constexpr int ACC_STRIDE = 256;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* b_full = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
-  uint64_t* b_empty = b_full + L::kNB;
-  uint64_t* a_full = b_empty + L::kNB;
-  uint64_t* a_empty = a_full + L::kNA;
-  uint64_t* tmem_full = a_empty + L::kNA;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_x);
-    tma_prefetch_desc(&tmap_x_tail);
-    tma_prefetch_desc(&tmap_w);
-    if (p.extra_blocks) tma_prefetch_desc(&tmap_x2);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < L::kNB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < L::kNA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 256); }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int num_tiles = p.num_m_tiles;                 // one n-tile: Cout <= 128
-  const int taps_t = p.taps_t, cin_blocks = p.cin_blocks, extra = p.extra_blocks;
-  const int n_groups = taps_t * 3 * cin_blocks;        // (kt, kh, cb) activation stages of three k-blocks each
-  // The shortcut's single-k-block stages are spread evenly between the regular groups (shortcut block e after
-  // max(1, (e + 1) * n_groups / (extra + 1)) regular groups): back to back at the end of a tile they would shrink the activation ring's
-  // lookahead from 3 x 1536 to 3 x 512 MMA cycles, less than a TMA round trip.  All three roles walk the same schedule.
-  auto extras_after = [&](int gi, int e) {
-    if (e >= extra) return false;
-    const int pos = (e + 1) * n_groups / (extra + 1);       // in [0, n_groups): after that many regular groups, at least one
-    return (pos < 1 ? 1 : pos) == gi + 1;
-  };
-
-  if (warp == 0) {
-    // ------------------------- activation rows: one stage per (kt, kh, cb) + one per shortcut block
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int t_o, th, tw;
-        conv_tile(p, tile, t_o, th, tw);
-        const int w0 = tw * 256;
-        int gi = 0, e = 0;
-        for (int kt_ = 0; kt_ < taps_t; ++kt_) {
-          const int t_in = t_o * p.stride_t + kt_;
-          for (int kh_ = 0; kh_ < 3; ++kh_) {
-            const int h_in = th + kh_ - 1;
-            for (int cb = 0; cb < cin_blocks; ++cb, ++gi) {
-              mbar_wait(&b_empty[stage], phase ^ 1);
-              uint8_t* sb = smem + stage * L::kBBytes;
-              mbar_expect_tx(&b_full[stage], L::kBBytes);
-              tma_load_4d(sb, &tmap_x, &b_full[stage], cb * BLOCK_K, w0 - 1, h_in, t_in);
-              tma_load_4d(sb + 256 * 128, &tmap_x_tail, &b_full[stage], cb * BLOCK_K, w0 + 255, h_in, t_in);
-              if (++stage == L::kNB) { stage = 0; phase ^= 1; }
-              for (; extras_after(gi, e); ++e) {        // fused 1x1x1 shortcut: the block input at the output pixels
-                mbar_wait(&b_empty[stage], phase ^ 1);
-                mbar_expect_tx(&b_full[stage], 256 * 128);
-                tma_load_4d(smem + stage * L::kBBytes, &tmap_x2, &b_full[stage], e * BLOCK_K, w0, th, t_o);
-                if (++stage == L::kNB) { stage = 0; phase ^= 1; }
-              }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 3 || warp == 2) {
-    // ------------------------- weight k-blocks, in the order the MMA warp consumes them.  Two threads (warp 3: even
-    // k-blocks, warp 2 — the TMEM allocator, idle in the main loop — odd ones): one producer iteration (barrier poll,
-    // expect-tx, TMA issue) costs ~500 cycles, the k-block's MMAs 512
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t turn = warp == 3 ? 0u : 1u;
-      const int cin = p.cin;
-      auto load = [&](int kcol) {
-        if ((turn++ & 1u) == 0u) {
-          mbar_wait(&a_empty[stage], phase ^ 1);
-          mbar_expect_tx(&a_full[stage], L::kABytes);
-          tma_load_2d(smem + L::kAOffset + stage * L::kABytes, &tmap_w, &a_full[stage], kcol, 0);
-        }
-        if (++stage == L::kNA) { stage = 0; phase ^= 1; }
-      };
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int gi = 0, e = 0;
-        for (int g = 0; g < taps_t * 3; ++g)            // g = kt * 3 + kh
-          for (int cb = 0; cb < cin_blocks; ++cb, ++gi) {
-            for (int kw_ = 0; kw_ < 3; ++kw_) load((g * 3 + kw_) * cin + cb * BLOCK_K);
-            for (; extras_after(gi, e); ++e) load(taps_t * 9 * cin + e * BLOCK_K);
-          }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------- MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BLOCK_M, 256);
-      int bs = 0, as = 0, acc = 0;
-      uint32_t bph = 0, aph = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * ACC_STRIDE;
-        // (the issuing thread is the critical resource: constant-trip tap loop, one comparison per group for the shortcut
-        // schedule — see the CTA-pair W-reuse loop)
-        uint32_t first = 1;
-        int e = 0;
-        auto next_extra_pos = [&](int e_) {
-          if (e_ >= extra) return 0x7fffffff;
-          const int pos = (e_ + 1) * n_groups / (extra + 1);
-          return pos < 1 ? 1 : pos;
-        };
-        int extra_pos = next_extra_pos(0);
-        auto taps = [&](const int n_taps) {
-          mbar_wait(&b_full[bs], bph);
-          const uint64_t b_desc0 = umma_desc_kmajor_sw128(smem_u32(smem + bs * L::kBBytes));
-#pragma unroll
-          for (int kw_ = 0; kw_ < 3; ++kw_) {
-            if (kw_ < n_taps) {
-              mbar_wait(&a_full[as], aph);
-              tc_fence_after();
-              const uint64_t a_desc = umma_desc_kmajor_sw128(smem_u32(smem + L::kAOffset + as * L::kABytes));
-              // the tap's 256 operand rows start kw rows (of 128 B) into the stage.  The 128B swizzle is a function of the
-              // absolute shared-memory address (bits 4-6 ^= bits 7-9) for TMA writes and UMMA reads alike, so a start address
-              // that is not 1024-aligned needs nothing else: the descriptor's base-offset field stays 0 (setting it to the
-              // start row's phase was measured to read the wrong chunks).
-              const uint64_t b_desc = b_desc0 + uint64_t(kw_ * 8);
-#pragma unroll
-              for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                umma_bf16(d_tmem, a_desc + uint64_t(k * 2), b_desc + uint64_t(k * 2), idesc, first ? 0u : 1u);
-                first = 0;
-              }
-              umma_commit(&a_empty[as]);
-              if (++as == L::kNA) { as = 0; aph ^= 1; }
-            }
-          }
-          umma_commit(&b_empty[bs]);
-          if (++bs == L::kNB) { bs = 0; bph ^= 1; }
-        };
-        for (int gi = 0; gi < n_groups; ++gi) {
-          taps(3);
-          while (extra_pos == gi + 1) {
-            taps(1);
-            extra_pos = next_extra_pos(++e);
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------- epilogue: the generic kernel's swap-AB epilogue (lanes = channels, columns = pixels)
-    const int q = warp & 3, half = (warp - 4) >> 2, row = q * 32 + lane;
-    uint8_t* slab = smem + L::kStagingOffset + (warp - 4) * 4096;
-    const int epi = p.epi;
-    const __nv_bfloat16* __restrict__ bias = p.bias;
-    const __nv_bfloat16* __restrict__ resid = p.residual;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int t_o, th, tw;
-      conv_tile(p, tile, t_o, th, tw);
-      const int r = th * p.tiles_w + tw;
-      const int w0 = tw * 256;
-      const float bsc = ((epi & EPI_BIAS) && row < p.N) ? __bfloat162float(bias[row]) : 0.f;
-      const long long fbase = (long long)(t_o + p.out_t_pad) * p.out_frame_stride + q * 32;
-      const bool dup_t = p.out_dup_head && t_o == 0;
-      mbar_wait_backoff(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (uint32_t(q * 32) << 16) + acc * ACC_STRIDE;
-      unsigned short* slab16 = reinterpret_cast<unsigned short*>(slab);
-      float4 st = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 1
-      for (int c0 = half * 128; c0 < half * 128 + 128; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(t_addr + c0, v);
-        tmem_ld_wait();
-        if (c0 + 32 >= half * 128 + 128) {
-          tc_fence_before();
-          mbar_arrive(&tmem_empty[acc]);
-        }
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          slab16[j * 64 + lane] = (unsigned short)(__float_as_uint(bf16_rne(__uint_as_float(v[j]) + bsc)) >> 16);
-        __syncwarp();
-        const int chn = lane & 3, psub = lane >> 2;
-        long long off[4];
-        int flags[4];
-        uint4 rv[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int w = w0 + c0 + i * 8 + psub;
-          const bool ok = (w < p.W_out) && (q * 32 + chn * 8 < p.N);
-          off[i] = fbase + ((long long)th * p.W_out + w) * p.ldc + chn * 8;
-          flags[i] = ok ? (dup_t ? 3 : 1) : 0;
-          if ((epi & EPI_RESIDUAL) && ok) rv[i] = *reinterpret_cast<const uint4*>(resid + off[i]);
-        }
-        __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(p.out);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          if (!(flags[i] & 1)) continue;
-          uint4 d = *reinterpret_cast<const uint4*>(slab + (i * 8 + psub) * 128 + chn * 16);
-          if (epi & EPI_RESIDUAL) {
-            const uint32_t dw[4] = {d.x, d.y, d.z, d.w}, rw[4] = {rv[i].x, rv[i].y, rv[i].z, rv[i].w};
-            uint32_t o[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              o[e] = pack_bf16x2(__uint_as_float(dw[e] << 16) + __uint_as_float(rw[e] << 16),
-                                 __uint_as_float(dw[e] & 0xffff0000u) + __uint_as_float(rw[e] & 0xffff0000u));
-            d = make_uint4(o[0], o[1], o[2], o[3]);
-          }
-          *reinterpret_cast<uint4*>(ob + off[i]) = d;
-          if (p.stat_partial) stat_acc(st, d);
-          if (flags[i] & 2) {
-            *reinterpret_cast<uint4*>(ob + off[i] - p.out_frame_stride) = d;
-            *reinterpret_cast<uint4*>(ob + off[i] - 2 * p.out_frame_stride) = d;
-          }
-        }
-        __syncwarp();
-      }
-      if (p.stat_partial) {
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          st.x += __shfl_xor_sync(0xffffffffu, st.x, o); st.y += __shfl_xor_sync(0xffffffffu, st.y, o);
-          st.z += __shfl_xor_sync(0xffffffffu, st.z, o); st.w += __shfl_xor_sync(0xffffffffu, st.w, o);
-        }
-        if (lane < 4 && t_o < p.T_out) {
-          const int octet = (q * 32) / 8 + lane;
-          if (octet * 8 < p.N) p.stat_partial[((long long)t_o * p.stat_slots + r * 2 + half) * (p.N / 8) + octet] = st;
-        }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
-
-template <int BLOCK_N, int KIND, bool SWAP = false, bool TWO = false, int EPI_CT = -1, bool WR = false>
+template <int BLOCK_N, int KIND, bool SWAP = false, int EPI_CT = -1>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p_in, cudaStream_t stream,
-                       const CUtensorMap* ta2_opt = nullptr, const CUtensorMap* tail_opt = nullptr) {
+                       const CUtensorMap* ta2_opt = nullptr) {
   const CUtensorMap& ta2 = ta2_opt ? *ta2_opt : ta;
-  const CUtensorMap& tail = tail_opt ? *tail_opt : ta;
-  using L = SmemLayout<BLOCK_N, TWO>;
-  auto kern = gemm_tcgen05_kernel<BLOCK_N, KIND, SWAP, TWO, EPI_CT, WR>;
+  using L = SmemLayout<BLOCK_N>;
+  auto kern = gemm_wgmma_kernel<BLOCK_N, KIND, SWAP, EPI_CT>;
   GemmParams p = p_in;
   {
-    // raster group: keep the group's B slice around 24 MB (L2 = 126 MB, shared with A tiles and the output stream)
+    // raster group: keep the group's B slice around 16 MB (L2 = 50 MB, shared with A tiles and the output stream)
     const long long b_tile_bytes = (long long)(SWAP ? BLOCK_M : BLOCK_N) * p.num_k_blocks * BLOCK_K * 2;
-    long long g = (24LL << 20) / (b_tile_bytes > 0 ? b_tile_bytes : 1);
+    long long g = (16LL << 20) / (b_tile_bytes > 0 ? b_tile_bytes : 1);
     if (g < 1) g = 1;
     if (g > p.num_n_tiles) g = p.num_n_tiles;
     p.group_n = (int)g;
@@ -1504,59 +1017,18 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmP
     if (e != cudaSuccess) return set_error(SVR2_ERR_CUDA, cudaGetErrorString(e));
     configured[dev] = true;
   }
-  if constexpr (TWO) {
-    const int tiles = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-    int clusters = num_sms() / 2;
-    if (tiles < clusters) clusters = tiles;
-    if (clusters <= 0) return SVR2_OK;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * clusters);
-    cfg.blockDim = dim3(kNumThreads);
-    cfg.dynamicSmemBytes = L::kTotal;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, ta2, tail, p);
-    if (e != cudaSuccess) return set_error(SVR2_ERR_CUDA, cudaGetErrorString(e));
-    return SVR2_OK;
-  } else {
-    int tiles = p.num_m_tiles * p.num_n_tiles;
-    int grid = tiles < num_sms() ? tiles : num_sms();
-    if (grid <= 0) return SVR2_OK;
-    kern<<<grid, kNumThreads, L::kTotal, stream>>>(ta, tb, ta2, tail, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(SVR2_ERR_CUDA, cudaGetErrorString(e));
-    return SVR2_OK;
-  }
-}
-
-// 0 = single-CTA tiles, 1 = CTA pairs (cta_group::2) for the 256/128-column kernels; SVR2_CTA_PAIR overrides
-static int g_pair_mode = -1;
-static int pair_mode() {
-  if (g_pair_mode < 0) {
-    const char* e = getenv("SVR2_CTA_PAIR");
-    g_pair_mode = e ? atoi(e) : 1;   // default: CTA pairs for the 256-column kernels (+9..14 % measured)
-  }
-  return g_pair_mode;
-}
-extern "C" void svr2_set_cta_pair(int on) { g_pair_mode = on ? 1 : 0; }
-
-// pair tiles are used for the 256/128-column bf16 / SwiGLU kernels when there are at least two m-tiles
-static bool want_pair(int block_n, int epi, int num_m_tiles) {
-  if (!pair_mode() || num_m_tiles < 2) return false;
-  (void)epi;
-  return block_n == 256;   // 128-column pair tiles lose to swap-AB (855-1042 vs ~1400 TFLOP/s measured)
+  int tiles = p.num_m_tiles * p.num_n_tiles;
+  int grid = tiles < num_sms() ? tiles : num_sms();
+  if (grid <= 0) return SVR2_OK;
+  kern<<<grid, kNumThreads, L::kTotal, stream>>>(ta, tb, ta2, p);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(SVR2_ERR_CUDA, cudaGetErrorString(e));
+  return SVR2_OK;
 }
 
 static int dispatch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
-                         cudaStream_t s, bool pair = false, const CUtensorMap* ta2 = nullptr) {
+                         cudaStream_t s, const CUtensorMap* ta2 = nullptr) {
   if (ta2) {     // conv with a fused shortcut: plain bf16 epilogue only
-    if (pair) return launch_gemm<256, KIND_BF16, false, true>(ta, tb, p, s, ta2);
     switch (block_n) {
       case 256: return launch_gemm<256, KIND_BF16>(ta, tb, p, s, ta2);
       case 128: return launch_gemm<128, KIND_BF16>(ta, tb, p, s, ta2);
@@ -1564,28 +1036,13 @@ static int dispatch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& 
     return set_error(SVR2_ERR_ARG, "fused shortcut: Cout must be >= 128");
   }
   if (p.epi & EPI_ROWSCALE) {
-    if (pair) return launch_gemm<256, KIND_BF16_RS, false, true>(ta, tb, p, s);
     if (block_n == 256) return launch_gemm<256, KIND_BF16_RS>(ta, tb, p, s);
     if (block_n == 128) return launch_gemm<128, KIND_BF16_RS>(ta, tb, p, s);
     return set_error(SVR2_ERR_ARG, "EPI_ROWSCALE needs >= 128-column tiles");
   }
   if ((p.epi & EPI_PEXP) && p.stat2) {
     if (block_n != 256) return set_error(SVR2_ERR_ARG, "EPI_PEXP statistics need 256-column tiles");
-    return pair ? launch_gemm<256, KIND_PEXP_STAT, false, true>(ta, tb, p, s) : launch_gemm<256, KIND_PEXP_STAT>(ta, tb, p, s);
-  }
-  if (pair) {
-    if (p.epi & EPI_SWIGLU) return launch_gemm<256, KIND_SWIGLU, false, true>(ta, tb, p, s);
-    if (p.epi & EPI_ROWSTAT) return launch_gemm<256, KIND_ROWSTAT, false, true>(ta, tb, p, s);
-    if (p.epi & EPI_PEXP) return launch_gemm<256, KIND_PEXP, false, true>(ta, tb, p, s);
-    if (p.epi & EPI_F32) return launch_gemm<256, KIND_F32, false, true>(ta, tb, p, s);
-    switch (p.epi) {      // the epilogue-bound shapes of the hot path get flag-free epilogues
-      case EPI_SHUFFLE | EPI_BIAS: return launch_gemm<256, KIND_BF16, false, true, EPI_SHUFFLE | EPI_BIAS>(ta, tb, p, s);
-      case EPI_BIAS | EPI_GATE | EPI_RESIDUAL: return launch_gemm<256, KIND_BF16, false, true, EPI_BIAS | EPI_GATE | EPI_RESIDUAL>(ta, tb, p, s);
-      case EPI_GATE | EPI_RESIDUAL: return launch_gemm<256, KIND_BF16, false, true, EPI_GATE | EPI_RESIDUAL>(ta, tb, p, s);
-      case EPI_BIAS: return launch_gemm<256, KIND_BF16, false, true, EPI_BIAS>(ta, tb, p, s);
-      case 0: return launch_gemm<256, KIND_BF16, false, true, 0>(ta, tb, p, s);
-    }
-    return launch_gemm<256, KIND_BF16, false, true>(ta, tb, p, s);
+    return launch_gemm<256, KIND_PEXP_STAT>(ta, tb, p, s);
   }
   if (p.epi & EPI_SWIGLU) {
     if (block_n == 256) return launch_gemm<256, KIND_SWIGLU>(ta, tb, p, s);
@@ -1610,6 +1067,15 @@ static int dispatch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& 
       case 64: return launch_gemm<64, KIND_F32>(ta, tb, p, s);
       case 32: return launch_gemm<32, KIND_F32>(ta, tb, p, s);
       case 16: return launch_gemm<16, KIND_F32>(ta, tb, p, s);
+    }
+  }
+  if (block_n == 256) {
+    switch (p.epi) {      // the epilogue-bound shapes of the hot path get flag-free epilogues
+      case EPI_SHUFFLE | EPI_BIAS: return launch_gemm<256, KIND_BF16, false, EPI_SHUFFLE | EPI_BIAS>(ta, tb, p, s);
+      case EPI_BIAS | EPI_GATE | EPI_RESIDUAL: return launch_gemm<256, KIND_BF16, false, EPI_BIAS | EPI_GATE | EPI_RESIDUAL>(ta, tb, p, s);
+      case EPI_GATE | EPI_RESIDUAL: return launch_gemm<256, KIND_BF16, false, EPI_GATE | EPI_RESIDUAL>(ta, tb, p, s);
+      case EPI_BIAS: return launch_gemm<256, KIND_BF16, false, EPI_BIAS>(ta, tb, p, s);
+      case 0: return launch_gemm<256, KIND_BF16, false, 0>(ta, tb, p, s);
     }
   }
   switch (block_n) {
@@ -1685,9 +1151,8 @@ static int linear_impl(const void* a, int64_t lda, const void* w, int64_t ldw, i
   uint32_t ba[2] = {BLOCK_K, BLOCK_M};
   int rc = make_tmap_bf16(&ta, a, 2, da, sa, ba);
   if (rc) return rc;
-  const bool pair = want_pair(bn, epi_flags, (M + BLOCK_M - 1) / BLOCK_M);
   uint64_t db[2] = {(uint64_t)K, (uint64_t)N}, sb[1] = {(uint64_t)ldw * 2};
-  uint32_t bb[2] = {BLOCK_K, (uint32_t)(pair ? bn / 2 : bn)};
+  uint32_t bb[2] = {BLOCK_K, (uint32_t)bn};
   rc = make_tmap_bf16(&tb, w, 2, db, sb, bb);
   if (rc) return rc;
   GemmParams p{};
@@ -1716,7 +1181,7 @@ static int linear_impl(const void* a, int64_t lda, const void* w, int64_t ldw, i
   p.stat2 = reinterpret_cast<float2*>(stat_out);
   p.ld_stat = (int)ld_stat;
   p.run_if = run_if;
-  return dispatch_gemm(bn, ta, tb, p, (cudaStream_t)stream, pair);
+  return dispatch_gemm(bn, ta, tb, p, (cudaStream_t)stream);
 }
 
 // QKV projection with NaSwinAttention's q/k RMSNorm + RoPE + window partition fused into the epilogue
@@ -1732,14 +1197,13 @@ extern "C" int svr2_linear_qkv_rope_bf16(const void* a, int64_t lda, const void*
   if ((lda % 8) || (ldw % 8)) return set_error(SVR2_ERR_ARG, "svr2_linear_qkv_rope_bf16: lda/ldw must be multiples of 8");
   const int inner = heads * 128, N = 3 * inner, bn = 256;
   const int num_m = (M + BLOCK_M - 1) / BLOCK_M;
-  const bool pair = want_pair(bn, 0, num_m);
   CUtensorMap ta, tb;
   uint64_t da[2] = {(uint64_t)K, (uint64_t)M}, sa[1] = {(uint64_t)lda * 2};
   uint32_t ba[2] = {BLOCK_K, BLOCK_M};
   int rc = make_tmap_bf16(&ta, a, 2, da, sa, ba);
   if (rc) return rc;
   uint64_t db[2] = {(uint64_t)K, (uint64_t)N}, sb[1] = {(uint64_t)ldw * 2};
-  uint32_t bb[2] = {BLOCK_K, (uint32_t)(pair ? bn / 2 : bn)};
+  uint32_t bb[2] = {BLOCK_K, (uint32_t)bn};
   rc = make_tmap_bf16(&tb, w, 2, db, sb, bb);
   if (rc) return rc;
   GemmParams p{};
@@ -1753,8 +1217,8 @@ extern "C" int svr2_linear_qkv_rope_bf16(const void* a, int64_t lda, const void*
   p.rope_cos = cos_tab; p.rope_sin = sin_tab;
   p.qk_weight = qk_weight; p.qk_eps = eps; p.qkv_inner = inner;
   cudaStream_t s = (cudaStream_t)stream;
-  if (nfreq == 21) return pair ? launch_gemm<256, KIND_QKV21, false, true>(ta, tb, p, s) : launch_gemm<256, KIND_QKV21>(ta, tb, p, s);
-  return pair ? launch_gemm<256, KIND_QKV10, false, true>(ta, tb, p, s) : launch_gemm<256, KIND_QKV10>(ta, tb, p, s);
+  if (nfreq == 21) return launch_gemm<256, KIND_QKV21>(ta, tb, p, s);
+  return launch_gemm<256, KIND_QKV10>(ta, tb, p, s);
 }
 
 // number of (max, sum) float2 partial slots per row that EPI_ROWSTAT writes for a given N
@@ -1808,31 +1272,6 @@ extern "C" int svr2_conv3d_shortcut_stats_bf16(const void* x, int T_in_total, in
 
 // Output tile of the implicit-GEMM conv.  Cout <= 128: swap operands (128 channels x 256 pixels per tile); else
 // 128 pixels x up to 256 channels.  bw x bh output pixels (128, or 256 when swapped).
-// W-reuse conv (conv_wreuse_kernel): activation maps with 256- and 8-pixel row boxes; the weight map (box 64 x 128 rows) and
-// the shortcut tensor's map (box 64 x 256 pixels) are the generic kernel's.
-static int launch_conv_wreuse(const void* x, int T_in_total, int H, int W, int Cin, const CUtensorMap& tw, const GemmParams& p,
-                              cudaStream_t stream, const CUtensorMap* tx2);
-
-// SVR2_CONV_WR / svr2_set_conv_wreuse: 0 off; 1 (default) W-reuse tiles (256 x 1 pixels) for swap-AB convs whose rows split
-// into 256-pixel segments with <= 4 % waste; 2 whenever a row holds a segment, CTA-pair kernels included (tests of the
-// ragged last segment); 3 = 1 + the CTA-pair kernels under the same waste rule
-static int g_conv_wr = -1;
-static int conv_wr_mode() {
-  if (g_conv_wr < 0) {
-    const char* e = getenv("SVR2_CONV_WR");
-    g_conv_wr = e ? atoi(e) : 1;
-  }
-  return g_conv_wr;
-}
-// CTA-pair kernels (Cout >= 256): the W-reuse mainloop is opt-in (mode 3, or 2 = everywhere for the tests): it lowers the
-// L2 -> SM traffic by a third and runs at 94.9 % tensor-pipe activity instead of 97.5 %, +1.8 % in isolation, no difference
-// in the 4K step (2614 vs 2621 ms) — the generic pair tiles stay the default
-static int conv_wr_pair_mode() {
-  const int m = conv_wr_mode();
-  return m == 2 ? 2 : (m == 3 ? 1 : 0);
-}
-extern "C" void svr2_set_conv_wreuse(int mode) { g_conv_wr = mode < 0 ? 0 : (mode > 3 ? 3 : mode); }
-
 static void conv_tile_shape(int Cout, int H_out, int W_out, bool* swap_out, int* bw_out, int* bh_out) {
   const bool swap = (Cout > 64 && Cout <= 128) && (long long)H_out * W_out >= 256;
   int bw = 16, bh = 8;
@@ -1840,19 +1279,9 @@ static void conv_tile_shape(int Cout, int H_out, int W_out, bool* swap_out, int*
     bw = 32; bh = 8;
     if (W_out <= 16) { bw = 16; bh = 16; }
     if (W_out <= 8) { bw = 8; bh = 32; }
-    const int seg = (W_out + 255) / 256;
-    if (conv_wr_mode() && W_out >= 256 && (conv_wr_mode() == 2 || (long long)seg * 256 * 100 <= (long long)W_out * 104)) {
-      bw = 256; bh = 1;      // SVR2_CONV_WR=2: whenever a row holds one segment (tests of the ragged last segment)
-    }
   } else {
     if (W_out >= 128 && H_out < 8) { bw = 128; bh = 1; }
     else if (W_out <= 8) { bw = 8; bh = 16; }
-    // CTA-pair W-reuse mainloop (Cout >= 256): m-tiles of one 128-pixel row segment, same waste rule
-    const int seg = (W_out + 127) / 128;
-    if (conv_wr_pair_mode() && Cout >= 256 && W_out >= 128 &&
-        (conv_wr_pair_mode() == 2 || (long long)seg * 128 * 100 <= (long long)W_out * 104)) {
-      bw = 128; bh = 1;
-    }
   }
   *swap_out = swap; *bw_out = bw; *bh_out = bh;
 }
@@ -1902,10 +1331,8 @@ static int conv3d_impl(const void* x, int T_in_total, int H, int W, int Cin, con
     if (rc) return rc;
   }
   const int K = kt * kh * kw * Cin + (x2 ? C2 : 0);
-  const int n_m_tiles = T_out * ((W_out + bw - 1) / bw) * ((H_out + bh - 1) / bh);
-  const bool pair = !swap && want_pair(bn, 0, n_m_tiles);
   uint64_t db[2] = {(uint64_t)K, (uint64_t)Cout}, sb[1] = {(uint64_t)K * 2};
-  uint32_t bb[2] = {BLOCK_K, (uint32_t)(pair ? bn / 2 : bn)};
+  uint32_t bb[2] = {BLOCK_K, (uint32_t)bn};
   rc = make_tmap_bf16(&tb, w, 2, db, sb, bb);
   if (rc) return rc;
   GemmParams p{};
@@ -1955,50 +1382,8 @@ static int conv3d_impl(const void* x, int T_in_total, int H, int W, int Cin, con
     p.stat_partial = (float4*)stat_partial;
     p.stat_slots = slots;
   }
-  if (swap && bw == 256 && bh == 1 && stride_hw == 1 && kh == 3 && kw == 3 && pad_hw == 1 && Cout <= 128 && Cout % 8 == 0)
-    return launch_conv_wreuse(x, T_in_total, H, W, Cin, tb, p, (cudaStream_t)stream, x2 ? &ta2 : nullptr);
   if (swap) return launch_gemm<256, KIND_BF16, true>(ta, tb, p, (cudaStream_t)stream, x2 ? &ta2 : nullptr);
-  if (pair && bn == 256 && bw == 128 && bh == 1 && stride_hw == 1 && kh == 3 && kw == 3 && pad_hw == 1 && conv_wr_pair_mode()) {
-    CUtensorMap tail;            // 8-pixel boxes behind the 128-pixel row segment (the kw = 1, 2 taps' last pixels)
-    uint64_t d[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)T_in_total};
-    uint64_t s4[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-    uint32_t b_tail[4] = {BLOCK_K, 8, 1, 1};
-    rc = make_tmap_bf16(&tail, x, 4, d, s4, b_tail);
-    if (rc) return rc;
-    return launch_gemm<256, KIND_BF16, false, true, -1, true>(ta, tb, p, (cudaStream_t)stream, x2 ? &ta2 : nullptr, &tail);
-  }
-  return dispatch_gemm(bn, ta, tb, p, (cudaStream_t)stream, pair, x2 ? &ta2 : nullptr);
-}
-
-static int launch_conv_wreuse(const void* x, int T_in_total, int H, int W, int Cin, const CUtensorMap& tw, const GemmParams& p,
-                              cudaStream_t stream, const CUtensorMap* tx2) {
-  CUtensorMap tx, tail;
-  uint64_t d[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)T_in_total};
-  uint64_t s[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-  uint32_t b_row[4] = {BLOCK_K, 256, 1, 1}, b_tail[4] = {BLOCK_K, 8, 1, 1};
-  int rc = make_tmap_bf16(&tx, x, 4, d, s, b_row);
-  if (rc) return rc;
-  rc = make_tmap_bf16(&tail, x, 4, d, s, b_tail);
-  if (rc) return rc;
-  // ring split (activation stages, weight stages): 3 + 5 (default) or 4 + 3 (SVR2_CONV_WR_RING=43, A/B)
-  static int ring = -1;
-  if (ring < 0) {
-    const char* e = getenv("SVR2_CONV_WR_RING");
-    ring = e ? atoi(e) : 35;
-  }
-  static bool configured[kMaxDevices] = {};
-  const int dev = current_device();
-  const int smem = ring == 43 ? WrSmem<4, 3>::kTotal : WrSmem<3, 5>::kTotal;
-  auto kern = ring == 43 ? conv_wreuse_kernel<4, 3> : conv_wreuse_kernel<3, 5>;
-  if (!configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(SVR2_ERR_CUDA, cudaGetErrorString(e));
-    configured[dev] = true;
-  }
-  const int grid = p.num_m_tiles < num_sms() ? p.num_m_tiles : num_sms();
-  if (grid <= 0) return SVR2_OK;
-  kern<<<grid, kNumThreads, smem, stream>>>(tx, tail, tw, tx2 ? *tx2 : tx, p);
-  return check_launch("conv_wreuse");
+  return dispatch_gemm(bn, ta, tb, p, (cudaStream_t)stream, x2 ? &ta2 : nullptr);
 }
 
 // Upsample3D: 1x1x1 conv (GEMM over voxels) with the 3-D pixel shuffle fused into the store.
@@ -2015,9 +1400,8 @@ extern "C" int svr2_upsample_shuffle_bf16(const void* x, int F, int H, int W, in
   uint32_t ba[2] = {BLOCK_K, BLOCK_M};
   int rc = make_tmap_bf16(&ta, x, 2, da, sa, ba);
   if (rc) return rc;
-  const bool pair = want_pair(bn, 0, (M + BLOCK_M - 1) / BLOCK_M);
   uint64_t db[2] = {(uint64_t)C, (uint64_t)N}, sb[1] = {(uint64_t)C * 2};
-  uint32_t bb[2] = {BLOCK_K, (uint32_t)(pair ? bn / 2 : bn)};
+  uint32_t bb[2] = {BLOCK_K, (uint32_t)bn};
   rc = make_tmap_bf16(&tb, w, 2, db, sb, bb);
   if (rc) return rc;
   GemmParams p{};
@@ -2035,5 +1419,5 @@ extern "C" int svr2_upsample_shuffle_bf16(const void* x, int F, int H, int W, in
   p.shuf_drop = (temporal && drop_head) ? 1 : 0;
   p.bias = (const __nv_bfloat16*)bias;
   p.out = y;
-  return dispatch_gemm(bn, ta, tb, p, (cudaStream_t)stream, pair);
+  return dispatch_gemm(bn, ta, tb, p, (cudaStream_t)stream);
 }

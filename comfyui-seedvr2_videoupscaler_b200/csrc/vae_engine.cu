@@ -348,7 +348,7 @@ struct Run {
       linear(P(y.off), C, wv->ptr, C, (int)tn, C, C, 0, bv->ptr, nullptr, nullptr, P(v), C, 1.f);
     }
     drop(y);
-    const long long wave_rows = 74 * 128;       // 74 m-tiles x 2 n-tiles (d = 512) = one full wave of 148 CTAs
+    const long long wave_rows = 66 * 128;       // 66 m-tiles x 2 n-tiles (d = 512) = one full wave of 132 CTAs
     long long kk = (1LL << 32) / (wave_rows * ldn * 2);
     if (kk < 1) kk = 1;
     long long cq = wave_rows * kk;

@@ -1,4 +1,4 @@
-"""Host side of the B200 NaDiT forward (3B and 7B).
+"""Host side of the H100 NaDiT forward (3B and 7B).
 
 Mirrors the reference operator interface ``NaDiT.forward(vid, txt, vid_shape,
 txt_shape, timestep) -> NaDiTOutput.vid_sample`` (reference

@@ -33,8 +33,6 @@ class TensorDesc(ctypes.Structure):
 _P = c_void_p
 SIGNATURES = {
     "svr2_version": [],
-    "svr2_set_cta_pair": [c_int],
-    "svr2_set_conv_wreuse": [c_int],
     "svr2_device_check": [POINTER(c_int), POINTER(c_int), POINTER(c_int)],
     "svr2_create": [POINTER(c_void_p), c_int, POINTER(ModelDesc)],
     "svr2_destroy": [_P],
@@ -118,7 +116,7 @@ def load() -> ctypes.CDLL:
         lib.svr2_engine_last_error.argtypes = [c_void_p]
         for name, args in SIGNATURES.items():
             fn = getattr(lib, name)
-            fn.restype = c_int64 if (name.endswith("_bytes") or name == "svr2_vae_last_launches") else (None if name in ("svr2_set_cta_pair", "svr2_set_conv_wreuse", "svr2_destroy") else c_int)
+            fn.restype = c_int64 if (name.endswith("_bytes") or name == "svr2_vae_last_launches") else (None if name == "svr2_destroy" else c_int)
             fn.argtypes = args
         _lib = lib
     return _lib

@@ -1,4 +1,4 @@
-"""Clip-level runner over the B200 engines.
+"""Clip-level runner over the H100 engines.
 
 Mirrors ``VideoDiffusionInfer`` (reference ``src/core/infer.py``): ``vae_encode``
 (:117-199), ``inference`` (:315-395, one Euler step, cfg = 1: x0 = x_t - v,

@@ -1,4 +1,4 @@
-"""Host side of the B200 causal 3-D conv video VAE (encode + decode).
+"""Host side of the H100 causal 3-D conv video VAE (encode + decode).
 
 Mirrors the reference operator interface
 ``VideoAutoencoderKLWrapper.encode(x).latent`` / ``.decode(z).sample``
@@ -222,7 +222,7 @@ class B200VideoVAE(EngineModule):
             elif k.endswith(".weight") and v.ndim == 5:
                 W[k] = self._conv_w(v)
             elif k.endswith(".weight") and v.ndim == 4:   # 2-D checkpoint: "tail" inflation (causal_inflation_lib.py:440-457)
-                raise NotImplementedError("2-D VAE checkpoints are not supported by the B200 engine")
+                raise NotImplementedError("2-D VAE checkpoints are not supported by the engine")
             else:
                 W[k] = self._vec(v) if v.ndim == 1 else v.to(self.device, torch.bfloat16).contiguous()
             if k.endswith(".weight") and v.ndim == 5:
@@ -376,7 +376,7 @@ class B200VideoVAE(EngineModule):
         #   pass 2: P = bf16(exp2(q k^T * scale - lse))  (normalised probabilities)
         #   then   O = P @ V  (V consumed through its transpose, K-major)
         ldn = (n + 7) // 8 * 8
-        wave_rows = 74 * 128                       # 74 m-tiles x 2 n-tiles (d = 512) = one full wave of 148 CTAs
+        wave_rows = 66 * 128                       # 66 m-tiles x 2 n-tiles (d = 512) = one full wave of 132 CTAs
         k = max(1, (1 << 32) // (wave_rows * ldn * 2))
         cq = min(wave_rows * k, (n + 127) // 128 * 128)
         slots = lib.load().svr2_rowstat_slots(n)

@@ -176,7 +176,7 @@ def load_state_dict(path: str, device="cpu") -> Dict[str, torch.Tensor]:
     ``src/core/model_loader.py:84-153``): ``.safetensors`` in fp16 / bf16 / fp32 or fp8_e4m3fn storage (the CLI default
     model is ``*_fp8_e4m3fn.safetensors``, ``model_registry.py:56``) and ``.pth`` / ``.pt``.  The engines cast every
     tensor to their bf16 / fp32 layouts on the GPU, so fp8 and fp16 storage need no separate path.  GGUF (block-quantised)
-    checkpoints are not part of the B200 path."""
+    checkpoints are not part of the engine's path."""
     low = path.lower()
     if low.endswith(".safetensors"):
         from safetensors.torch import load_file
@@ -186,7 +186,7 @@ def load_state_dict(path: str, device="cpu") -> Dict[str, torch.Tensor]:
         if isinstance(sd, dict) and "state_dict" in sd and all(not torch.is_tensor(v) for v in sd.values()):
             sd = sd["state_dict"]
     elif low.endswith(".gguf"):
-        raise NotImplementedError("GGUF checkpoints are not supported by the B200 engine (use the safetensors files)")
+        raise NotImplementedError("GGUF checkpoints are not supported by the engine (use the safetensors files)")
     else:
         raise ValueError(f"unknown checkpoint format: {path}")
     prefix = "model.diffusion_model."          # ComfyUI-style exports (model_loader.py:143-147)

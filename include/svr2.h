@@ -1,4 +1,4 @@
-/* libsvr2.so — C ABI of the B200-native SeedVR2 hot path (DiT forward + video-VAE).
+/* libsvr2.so — C ABI of the H100-native SeedVR2 hot path (DiT forward + video-VAE).
  *
  * Every entry point is `extern "C"`, takes plain device pointers / sizes and a
  * CUDA stream handle (`void*` = cudaStream_t, 0 = default stream); no torch types.
@@ -24,7 +24,7 @@ enum svr2_status {
   SVR2_OK = 0,
   SVR2_ERR_ARG = -1,   /* invalid argument / unsupported shape */
   SVR2_ERR_CUDA = -2,  /* CUDA runtime / driver error */
-  SVR2_ERR_ARCH = -3,  /* device is not sm_100 */
+  SVR2_ERR_ARCH = -3,  /* device is not sm_90 */
 };
 
 /* epilogue flags of svr2_linear_bf16 / svr2_conv3d_bf16 (applied in this order,
@@ -43,16 +43,8 @@ enum svr2_epilogue {
 };
 
 const char* svr2_last_error(void);
-/* 1: GEMM/conv tiles are executed by CTA pairs (tcgen05 cta_group::2, 256-row tiles); 0: single-CTA tiles.
- * Default from the environment variable SVR2_CTA_PAIR (unset = library default). */
-void svr2_set_cta_pair(int on);
-/* Stride-1 3x3 convs: 0 = generic tiles (32 x 8 / 16 x 8 pixels), 1 (default) = the W-reuse kernel for Cout <= 128 (tiles of
- * one 256-pixel row segment, the three horizontal taps read one activation stage) where rows split into segments with <= 4 %
- * waste, 2 = wherever a row holds a segment and also in the CTA-pair kernels (Cout >= 256, 128-pixel segments), 3 = 1 + the
- * CTA-pair kernels under the waste rule.  Default from SVR2_CONV_WR.  Changes svr2_conv_stat_slots(). */
-void svr2_set_conv_wreuse(int mode);
 int svr2_version(void);
-/* fills sm count / major / minor of the current device; SVR2_ERR_ARCH unless sm_100 */
+/* fills sm count / major / minor of the current device; SVR2_ERR_ARCH unless sm_90 */
 int svr2_device_check(int* sm_count, int* cc_major, int* cc_minor);
 
 /* ---- Handle-based engine API (SURVEY.md §8(b)): one svr2_t per (process, device); not thread-safe; all work is

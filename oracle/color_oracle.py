@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY — never imported by the product path.
 
 CPU restatement (plain torch) of the reference's post-decode colour correction
-(``src/utils/color_fix.py``) for the three methods the B200 engine ships:
+(``src/utils/color_fix.py``) for the three methods the engine ships:
 
   * ``wavelet``  — ``wavelet_reconstruction``            (``color_fix.py:122-246``)
   * ``adain``    — ``adaptive_instance_normalization``   (``color_fix.py:72-119``)
@@ -198,7 +198,7 @@ def merge_shards(chunks, overlap: int) -> torch.Tensor:
 
 
 # ---------------------------------------------------------------- HSV / wavelet-adaptive (round-2 groundwork)
-# The B200 engine does not ship these two modes yet (color_fix.apply_color_correction raises for them); the
+# The engine does not ship these two modes yet (color_fix.apply_color_correction raises for them); the
 # restatements below are pinned to the reference so that the kernels can be built against them next.
 def rgb_to_hsv(rgb01: torch.Tensor) -> torch.Tensor:
     """color_fix.py:614-649.  rgb [B,3,H,W] in [0,1] -> (h, s, v) in [0,1]; on channel ties the later of the

@@ -13,7 +13,7 @@ result back (``_functional_tensor.resize``); torch 2.11 ``_upsample_bicubic2d_aa
 Keys cubic (a = -0.5) whose support widens by the down-scale factor, weights normalised to sum 1.
 Pinned: ``oracle/make_golden.py`` runs the reference's own transform classes on CPU and checks this
 restatement against them (``tests/golden/pre_*.npz``); the GPU tests additionally compare the kernel with
-torch's CUDA ``interpolate`` on the B200 box.
+torch's CUDA ``interpolate`` on the GPU.
 """
 from __future__ import annotations
 

@@ -37,7 +37,7 @@ def cpu_vae(pkg):
     lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
     vae = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.vae")
     mp = pytest.MonkeyPatch()
-    mp.setattr(lib, "device_check", lambda: (148, 10, 0))
+    mp.setattr(lib, "device_check", lambda: (132, 9, 0))
     eng = vae.B200VideoVAE(pkg.weights.synth_vae_state_dict(seed=1, dtype=torch.float16), device="cpu")
     eng.native = False
     log = []

@@ -119,18 +119,16 @@ def _to_ndhwc(x_ncdhw, halo):
     (128, 128, (1, 3, 3), 1, 2, 2, 40, 72),      # swap-AB, spatial-only downsample
     (256, 128, (3, 3, 3), 1, 1, 2, 30, 44),      # swap-AB, ragged tile edges
     (128, 128, (1, 1, 1), 1, 1, 2, 24, 40),      # swap-AB 1x1x1
-    (128, 128, (3, 3, 3), 1, 1, 3, 9, 256),      # W-reuse kernel: one 256-pixel row segment per tile, 3 kw taps per load
-    (256, 128, (3, 3, 3), 1, 1, 2, 5, 520),      # W-reuse: three segments, ragged last one (8 valid pixels)
-    (128, 96, (1, 3, 3), 1, 1, 2, 6, 512),       # W-reuse: kt = 1, Cout < 128
-    (128, 128, (1, 3, 3), 1, 2, 2, 8, 1024),     # 256 x 1 tiles on the generic swap-AB kernel (stride 2: not eligible)
-    (256, 256, (3, 3, 3), 1, 1, 2, 6, 256),      # CTA-pair W-reuse mainloop: 128-pixel row segments, A descriptors shifted by kw rows
-    (256, 512, (3, 3, 3), 1, 1, 1, 3, 128),      # pair W-reuse: two n-tiles, odd number of m-tiles (phantom tile)
-    (512, 256, (1, 3, 3), 1, 1, 2, 5, 200),      # pair W-reuse: kt = 1, ragged second segment
-    (256, 256, (3, 3, 3), 2, 2, 3, 8, 512),      # 128 x 1 tiles on the generic pair kernel (stride 2: not eligible)
+    (128, 128, (3, 3, 3), 1, 1, 3, 9, 256),      # swap-AB, wide rows
+    (256, 128, (3, 3, 3), 1, 1, 2, 5, 520),      # swap-AB, wide rows, ragged last tile column
+    (128, 96, (1, 3, 3), 1, 1, 2, 6, 512),       # swap-AB, kt = 1, Cout < 128
+    (128, 128, (1, 3, 3), 1, 2, 2, 8, 1024),     # swap-AB, stride 2, wide rows
+    (256, 256, (3, 3, 3), 1, 1, 2, 6, 256),      # 256-column tiles, wide rows
+    (256, 512, (3, 3, 3), 1, 1, 1, 3, 128),      # two n-tiles, 128 x 1 pixel tiles (H_out < 8)
+    (512, 256, (1, 3, 3), 1, 1, 2, 5, 200),      # kt = 1, 128 x 1 pixel tiles, ragged second tile
+    (256, 256, (3, 3, 3), 2, 2, 3, 8, 512),      # 128 x 1 pixel tiles, stride 2
 ])
 def test_conv3d(svr2lib, Cin, Cout, k, st, shw, T, H, W):
-    if W >= 128:
-        svr2lib.load().svr2_set_conv_wreuse(2)        # W-reuse tiles also where the last row segment is mostly empty
     x = rnd(1, Cin, T, H, W, seed=1)
     w = rnd(Cout, Cin, *k, std=(Cin * k[0] * k[1] * k[2]) ** -0.5, seed=2)
     b = rnd(Cout, seed=3)
@@ -150,27 +148,17 @@ def test_conv3d(svr2lib, Cin, Cout, k, st, shw, T, H, W):
                    bias=bf(b), residual=torch.cat([res[:1], res[:1], res], 0).contiguous(), out_t_pad=2,
                    out_dup_head=1)
     ref_nd = bf(bf(ref[0].permute(1, 2, 3, 0)).float() + res.float())
-    svr2lib.load().svr2_set_conv_wreuse(1)
     assert_close(y[2:], ref_nd, 4e-3, "conv3d body")
     assert torch.equal(y[0], y[2]) and torch.equal(y[1], y[2]), "halo frames must replicate frame 0"
-    if W >= 128 and shw == 1 and k[1] == 3:           # the generic kernel on the same problem: same products,
-        y0 = torch.zeros_like(y)                      # another summation order of the fp32 accumulation
-        svr2lib.load().svr2_set_conv_wreuse(0)
-        try:
-            svr2lib.conv3d(x_nd, T + halo, H, W, Cin, w_k, Cout, k, st, shw, 1, T_out, y0, bias=bf(b),
-                           residual=torch.cat([res[:1], res[:1], res], 0).contiguous(), out_t_pad=2, out_dup_head=1)
-        finally:
-            svr2lib.load().svr2_set_conv_wreuse(1)
-        assert_close(y, y0, 2e-3, "W-reuse kernel vs generic swap-AB kernel")
 
 
 @pytest.mark.parametrize("Cin,C2,Cout,T,H,W", [
     (128, 256, 128, 2, 30, 44),     # decoder up3.res0: swap-AB, ragged tile edges
-    (256, 512, 256, 3, 24, 40),     # decoder up2.res0: CTA pair
+    (256, 512, 256, 3, 24, 40),     # decoder up2.res0: 256-column tiles
     (256, 128, 256, 2, 17, 33),     # encoder down1.res0 (odd sizes)
     (512, 256, 512, 1, 9, 16),      # encoder down2.res0, single frame
-    (128, 256, 128, 2, 7, 512),     # W-reuse kernel with the shortcut's extra k-blocks
-    (256, 512, 256, 2, 5, 256),     # CTA-pair W-reuse mainloop with the shortcut's extra k-blocks
+    (128, 256, 128, 2, 7, 512),     # swap-AB, wide rows, with the shortcut's extra k-blocks
+    (256, 512, 256, 2, 5, 256),     # 256-column tiles, wide rows, with the shortcut's extra k-blocks
 ])
 def test_conv3d_fused_shortcut(svr2lib, Cin, C2, Cout, T, H, W):
     """conv2(h) + conv_shortcut(x) as one contraction over [h ; x] (ResnetBlock3D, attn_video_vae.py:311-362) vs torch:

@@ -1,4 +1,4 @@
-"""Can an HBM-bound GroupNorm run concurrently with the persistent tcgen05 conv kernel (2 streams)?"""
+"""Can an HBM-bound GroupNorm run concurrently with the persistent wgmma conv kernel (2 streams)?"""
 import os, sys, importlib, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

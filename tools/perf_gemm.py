@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM / implicit-conv kernel on representative shapes
+"""Micro-benchmark of the wgmma GEMM / implicit-conv kernel on representative shapes
 (used for ncu captures and kernel tuning; not a pytest)."""
 import os, sys, importlib
 import torch
