@@ -22,28 +22,6 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-template <int kWarps>
-__device__ __forceinline__ float block_sum(float v, float* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float t = 0.f;
-#pragma unroll
-  for (int i = 0; i < kWarps; ++i) t += red[i];
-  __syncthreads();
-  return t;
-}
-template <int kWarps>
-__device__ __forceinline__ float block_max(float v, float* red) {
-  v = warp_max(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float t = -INFINITY;
-#pragma unroll
-  for (int i = 0; i < kWarps; ++i) t = fmaxf(t, red[i]);
-  __syncthreads();
-  return t;
-}
 
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   const uint32_t w[4] = {u.x, u.y, u.z, u.w};
@@ -132,66 +110,6 @@ __global__ void __launch_bounds__(256) rmsnorm_ada_kernel(const __nv_bfloat16* _
 // ------------------------------------------------------------------ q/k norm + RoPE + window gather
 // one block per output row (window-ordered); warp w handles heads w, w+nwarps, ...; lane = 4 dims.
 __global__ void __launch_bounds__(256) qk_norm_rope_window_kernel(
-    const __nv_bfloat16* __restrict__ qkv_vid, const __nv_bfloat16* __restrict__ qkv_txt,
-    const int32_t* __restrict__ row_src, const int32_t* __restrict__ row_rope, const float* __restrict__ cos_tab,
-    const float* __restrict__ sin_tab, int nfreq, const float* __restrict__ wq_vid, const float* __restrict__ wk_vid,
-    const float* __restrict__ wq_txt, const float* __restrict__ wk_txt, float eps, int heads,
-    __nv_bfloat16* __restrict__ q, __nv_bfloat16* __restrict__ k, __nv_bfloat16* __restrict__ v,
-    const int32_t* __restrict__ row_list) {
-  const long long r = row_list ? (long long)row_list[blockIdx.x] : (long long)blockIdx.x;   // optional subset of the rows
-  const int src = row_src[r];
-  const bool is_txt = src < 0;
-  const int inner = heads * 128;
-  const __nv_bfloat16* base = is_txt ? qkv_txt + (long long)(-src - 1) * 3 * inner : qkv_vid + (long long)src * 3 * inner;
-  const float* wq = is_txt ? wq_txt : wq_vid;
-  const float* wk = is_txt ? wk_txt : wk_vid;
-  const int ri[3] = {row_rope[r * 3 + 0], row_rope[r * 3 + 1], row_rope[r * 3 + 2]};
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const int d0 = lane * 4;
-  const int rot = 6 * nfreq;  // rotated dims
-  // per-lane cos/sin for the two pairs (d0,d0+1), (d0+2,d0+3)
-  float cs[2], sn[2];
-#pragma unroll
-  for (int pi = 0; pi < 2; ++pi) {
-    const int d = d0 + 2 * pi;
-    cs[pi] = 1.f;
-    sn[pi] = 0.f;
-    if (d < rot) {
-      const int axis = d / (2 * nfreq), j = (d % (2 * nfreq)) >> 1;
-      const int tr = ri[axis];
-      if (tr >= 0) {
-        cs[pi] = cos_tab[tr * nfreq + j];
-        sn[pi] = sin_tab[tr * nfreq + j];
-      }
-    }
-  }
-  const float4 wq4 = *reinterpret_cast<const float4*>(wq + d0);
-  const float4 wk4 = *reinterpret_cast<const float4*>(wk + d0);
-  for (int h = warp; h < heads; h += nwarps) {
-    const long long o_off = (r * heads + h) * 128 + d0;
-#pragma unroll
-    for (int which = 0; which < 2; ++which) {
-      const uint2 raw = *reinterpret_cast<const uint2*>(base + which * inner + h * 128 + d0);
-      const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&raw);
-      float2 a = __bfloat1622float2(hh[0]), b = __bfloat1622float2(hh[1]);
-      float ss = a.x * a.x + a.y * a.y + b.x * b.x + b.y * b.y;
-      ss = warp_sum(ss);
-      const float rr = 1.0f / sqrtf(ss * (1.0f / 128.0f) + eps);
-      const float4 w4 = which == 0 ? wq4 : wk4;
-      float x0 = a.x * rr * w4.x, x1 = a.y * rr * w4.y, x2 = b.x * rr * w4.z, x3 = b.y * rr * w4.w;
-      // interleaved-pair rotation: (x0,x1) -> (x0 c - x1 s, x1 c + x0 s)
-      const float y0 = x0 * cs[0] - x1 * sn[0], y1 = x1 * cs[0] + x0 * sn[0];
-      const float y2 = x2 * cs[1] - x3 * sn[1], y3 = x3 * cs[1] + x2 * sn[1];
-      uint2 outv = make_uint2(pack_bf16x2(y0, y1), pack_bf16x2(y2, y3));
-      *reinterpret_cast<uint2*>((which == 0 ? q : k) + o_off) = outv;
-    }
-    *reinterpret_cast<uint2*>(v + o_off) = *reinterpret_cast<const uint2*>(base + 2 * inner + h * 128 + d0);
-  }
-}
-
-// v2 of the kernel above (default; SVR2_QK_ROPE=v1 selects the first version): same arithmetic, q/k/v of up to three heads per warp fetched up front
-// one block per output row (window-ordered); warp w handles heads w, w+nwarps, ...; lane = 4 dims.
-__global__ void __launch_bounds__(256) qk_norm_rope_window_v2_kernel(
     const __nv_bfloat16* __restrict__ qkv_vid, const __nv_bfloat16* __restrict__ qkv_txt,
     const int32_t* __restrict__ row_src, const int32_t* __restrict__ row_rope, const float* __restrict__ cos_tab,
     const float* __restrict__ sin_tab, int nfreq, const float* __restrict__ wq_vid, const float* __restrict__ wk_vid,
@@ -455,73 +373,14 @@ __global__ void __launch_bounds__(256) groupnorm_finalize_fused_kernel(const flo
   }
 }
 
-__global__ void __launch_bounds__(256) groupnorm_apply_kernel(const __nv_bfloat16* __restrict__ x,
-                                                              __nv_bfloat16* __restrict__ y, int hw, int C, int silu,
-                                                              int out_t_pad, int out_dup_head,
-                                                              const float2* __restrict__ coef) {
-  const int f = blockIdx.y;
-  const int cvec = C / 8;
-  const long long nvec = (long long)hw * cvec;
-  const __nv_bfloat16* xf = x + (long long)f * hw * C;
-  __nv_bfloat16* yf = y + (long long)(f + out_t_pad) * hw * C;
-  // 256 % cvec == 0 and every stride below is a multiple of 256: a thread always owns the same 8 channels
-  const int cv = threadIdx.x % cvec;
-  float ca[8], cb[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float2 t = coef[(long long)f * C + cv * 8 + e];
-    ca[e] = t.x;
-    cb[e] = t.y;
-  }
-  const bool dup = out_dup_head && f == 0;
-  const long long stride = (long long)gridDim.x * 256;
-  long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-  for (; i + 3 * stride < nvec; i += 4 * stride) {
-    uint4 r[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) r[u] = __ldcs(reinterpret_cast<const uint4*>(xf) + i + u * stride);   // streamed once
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      float v[8], o[8];
-      unpack8(r[u], v);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float t = bf16_rne(v[e] * ca[e] + cb[e]);   // F.group_norm output is bf16
-        o[e] = silu ? silu_fast(t) : t;
-      }
-      const uint4 pk = pack8(o);
-      reinterpret_cast<uint4*>(yf)[i + u * stride] = pk;
-      if (dup) {
-        reinterpret_cast<uint4*>(yf - (long long)hw * C)[i + u * stride] = pk;
-        reinterpret_cast<uint4*>(yf - 2LL * hw * C)[i + u * stride] = pk;
-      }
-    }
-  }
-  for (; i < nvec; i += stride) {
-    float v[8], o[8];
-    unpack8(reinterpret_cast<const uint4*>(xf)[i], v);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const float t = bf16_rne(v[e] * ca[e] + cb[e]);
-      o[e] = silu ? silu_fast(t) : t;
-    }
-    const uint4 pk = pack8(o);
-    reinterpret_cast<uint4*>(yf)[i] = pk;
-    if (dup) {
-      reinterpret_cast<uint4*>(yf - (long long)hw * C)[i] = pk;
-      reinterpret_cast<uint4*>(yf - 2LL * hw * C)[i] = pk;
-    }
-  }
-}
-
-// Same arithmetic, leaner: the bf16 rounding of the normalised value is one cvt.rn.bf16x2 per channel pair (instead
-// of an integer round-to-nearest-even per value), six 16-byte loads in flight per thread and at most 64 registers
-// so that four blocks fit an SM — the kernel is latency-bound at the power-capped clock, not DRAM-bound.
+// The bf16 rounding of the normalised value is one cvt.rn.bf16x2 per channel pair, six 16-byte loads are in flight per
+// thread and at most 64 registers are used so that four blocks fit an SM — the kernel is latency-bound at the
+// power-capped clock, not DRAM-bound.
 template <bool SILU>
-__global__ void __launch_bounds__(256, 4) groupnorm_apply_v2_kernel(const __nv_bfloat16* __restrict__ x,
-                                                                    __nv_bfloat16* __restrict__ y, int hw, int C,
-                                                                    int out_t_pad, int out_dup_head,
-                                                                    const float2* __restrict__ coef) {
+__global__ void __launch_bounds__(256, 4) groupnorm_apply_kernel(const __nv_bfloat16* __restrict__ x,
+                                                                 __nv_bfloat16* __restrict__ y, int hw, int C,
+                                                                 int out_t_pad, int out_dup_head,
+                                                                 const float2* __restrict__ coef) {
   const int f = blockIdx.y;
   const int cvec = C / 8;
   const long long nvec = (long long)hw * cvec;
@@ -576,60 +435,17 @@ __global__ void __launch_bounds__(256, 4) groupnorm_apply_v2_kernel(const __nv_b
   }
 }
 
-// SVR2_GN_APPLY=v1 selects the first version (A/B measurements)
-static bool gn_apply_v2() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SVR2_GN_APPLY");
-    v = (e && e[0] == 'v' && e[1] == '1') ? 0 : 1;
-  }
-  return v != 0;
-}
 static void launch_gn_apply(const void* x, void* y, int frames, int hw, int C, int silu, int out_t_pad, int out_dup_head,
                             const float2* coef, cudaStream_t s) {
   const long long nvec = (long long)hw * C / 8;
-  if (gn_apply_v2()) {
-    int bx = (int)((nvec + 256 * 12 - 1) / (256 * 12));
-    if (bx < 1) bx = 1;
-    if (silu)
-      groupnorm_apply_v2_kernel<true><<<dim3(bx, frames), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, hw, C,
-                                                                       out_t_pad, out_dup_head, coef);
-    else
-      groupnorm_apply_v2_kernel<false><<<dim3(bx, frames), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, hw, C,
-                                                                        out_t_pad, out_dup_head, coef);
-  } else {
-    int bx = (int)((nvec + 256 * 8 - 1) / (256 * 8));
-    if (bx < 1) bx = 1;
-    groupnorm_apply_kernel<<<dim3(bx, frames), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, hw, C, silu,
-                                                            out_t_pad, out_dup_head, coef);
-  }
-}
-
-// ------------------------------------------------------------------ softmax rows fp32 -> bf16
-__global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ s, long long lds,
-                                                           __nv_bfloat16* __restrict__ p, long long ldp, int cols) {
-  __shared__ float red[8];
-  const float* sr = s + (long long)blockIdx.x * lds;
-  __nv_bfloat16* pr = p + (long long)blockIdx.x * ldp;
-  float m = -INFINITY;
-  for (int c = threadIdx.x * 4; c < cols; c += 1024) {
-    const float4 v = *reinterpret_cast<const float4*>(sr + c);
-    m = fmaxf(fmaxf(m, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
-  }
-  m = block_max<8>(m, red);
-  float sum = 0.f;
-  for (int c = threadIdx.x * 4; c < cols; c += 1024) {
-    const float4 v = *reinterpret_cast<const float4*>(sr + c);
-    sum += __expf(v.x - m) + __expf(v.y - m) + __expf(v.z - m) + __expf(v.w - m);
-  }
-  sum = block_sum<8>(sum, red);
-  const float inv = 1.0f / sum;
-  for (int c = threadIdx.x * 4; c < cols; c += 1024) {
-    const float4 v = *reinterpret_cast<const float4*>(sr + c);
-    uint2 o = make_uint2(pack_bf16x2(__expf(v.x - m) * inv, __expf(v.y - m) * inv),
-                         pack_bf16x2(__expf(v.z - m) * inv, __expf(v.w - m) * inv));
-    *reinterpret_cast<uint2*>(pr + c) = o;
-  }
+  int bx = (int)((nvec + 256 * 12 - 1) / (256 * 12));
+  if (bx < 1) bx = 1;
+  if (silu)
+    groupnorm_apply_kernel<true><<<dim3(bx, frames), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, hw, C,
+                                                                  out_t_pad, out_dup_head, coef);
+  else
+    groupnorm_apply_kernel<false><<<dim3(bx, frames), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, hw, C,
+                                                                   out_t_pad, out_dup_head, coef);
 }
 
 // ------------------------------------------------------------------ attention pass-1 combine
@@ -883,13 +699,7 @@ static int qk_norm_rope_launch(const void* qkv_vid, const void* qkv_txt, const i
   if (n_rows <= 0) return SVR2_OK;
   if (6 * nfreq > 128) return set_error(SVR2_ERR_ARG, "rope: 6*nfreq > head_dim");
   const int threads = heads >= 8 ? 256 : 32 * heads;   // 8 warps loop over the heads (one warp per head was slower: 54 vs 34 ms)
-  static int v2 = -1;
-  if (v2 < 0) {
-    const char* e = getenv("SVR2_QK_ROPE");
-    v2 = (e && e[0] == 'v' && e[1] == '1') ? 0 : 1;     // v2: 34.4 -> 30.2 ms per 4K step on the same box; SVR2_QK_ROPE=v1 for A/B
-  }
-  auto kern = v2 ? qk_norm_rope_window_v2_kernel : qk_norm_rope_window_kernel;
-  kern<<<n_rows, threads, 0, (cudaStream_t)stream>>>(
+  qk_norm_rope_window_kernel<<<n_rows, threads, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)qkv_vid, (const __nv_bfloat16*)qkv_txt, row_src, row_rope, cos_tab, sin_tab, nfreq, wq_vid,
       wk_vid, wq_txt, wk_txt, eps, heads, (__nv_bfloat16*)q, (__nv_bfloat16*)k, (__nv_bfloat16*)v, row_list);
   return check_launch("qk_norm_rope_window");
@@ -989,14 +799,6 @@ extern "C" int64_t svr2_groupnorm_scratch_bytes(int frames, int hw, int C) {
   long long blocks_x = (hw + 4095) / 4096;
   if (blocks_x < 1) blocks_x = 1;
   return (int64_t)(sizeof(double) * 64 * blocks_x * frames + sizeof(float2) * (long long)frames * C);
-}
-
-extern "C" int svr2_softmax_rows_bf16(const float* s, int64_t lds, void* p, int64_t ldp, int rows, int cols,
-                                      void* stream) {
-  if (cols % 4 || lds % 4 || ldp % 4) return set_error(SVR2_ERR_ARG, "softmax_rows: cols/lds/ldp % 4");
-  if (rows <= 0) return SVR2_OK;
-  softmax_rows_kernel<<<rows, 256, 0, (cudaStream_t)stream>>>(s, lds, (__nv_bfloat16*)p, ldp, cols);
-  return check_launch("softmax_rows");
 }
 
 extern "C" int svr2_rowstat_combine(const void* partial, int slots, int64_t ld, float* lse, int rows, void* stream) {

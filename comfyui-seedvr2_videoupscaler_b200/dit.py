@@ -188,12 +188,12 @@ class B200NaDiT(EngineModule):
         self._layouts: Dict[tuple, tuple] = {}
         self.attention = FlashAttentionVarlen()
         self._load(state_dict)
-        import os
         # the fused QKV epilogue needs 256-column tiles to be whole head pairs and one of the two shipped RoPE widths
-        self.fuse_qkv = (cfg["heads"] % 2 == 0 and os.environ.get("SVR2_FUSE_QKV", "1") != "0"
-                         and self.rope_freqs[0].numel() in (21, 10))
-        # forward sequenced by the native runtime (default) or by this module's Python loop (per-call profiling, A/B)
-        self.native = os.environ.get("SVR2_NATIVE_DIT", "1") != "0"
+        # (the same rule as fuse_qkv_ok in csrc/engine.cu)
+        self.fuse_qkv = cfg["heads"] % 2 == 0 and self.rope_freqs[0].numel() in (21, 10)
+        # forward sequenced by the native runtime (default) or by this module's Python loop (per-call profiling, tests
+        # against the native runtime)
+        self.native = True
 
     def _device_state_moved(self):
         if hasattr(self, "_layouts"):
@@ -376,7 +376,7 @@ class B200NaDiT(EngineModule):
         L = T * Hp * Wp
         vid = vid.to(dev, torch.bfloat16).contiguous()
         txt = txt.to(dev, torch.bfloat16).contiguous()
-        if self.native and lib.PROFILER is None and self.fuse_qkv == (cfg["heads"] % 2 == 0):
+        if self.native and lib.PROFILER is None:
             out = torch.empty(T * H * Wd, cfg["out_ch"], device=dev, dtype=torch.bfloat16)
             # the workspace comes from torch's caching allocator (and from the capture pool inside a CUDA graph) and goes
             # back to it after the forward: the VAE phases need those bytes (35 GB at a 65-frame 4K clip)

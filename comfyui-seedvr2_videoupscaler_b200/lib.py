@@ -68,7 +68,6 @@ SIGNATURES = {
     "svr2_unpatchify_bf16": [_P, c_int, _P, c_int, c_int, c_int, c_int, _P],
     "svr2_groupnorm_bf16": [_P, _P, c_int, c_int, c_int, _P, _P, c_float, c_int, c_int, c_int, _P, c_int64, _P],
     "svr2_groupnorm_scratch_bytes": [c_int, c_int, c_int],
-    "svr2_softmax_rows_bf16": [_P, c_int64, _P, c_int64, c_int, c_int, _P],
     "svr2_linear_ex_bf16": [_P, c_int64, _P, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int64, c_float, _P, _P,
                             c_int64, _P, _P],
     "svr2_rowstat_max": [_P, c_int, c_int64, _P, c_int, _P, _P],

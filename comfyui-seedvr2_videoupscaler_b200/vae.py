@@ -39,9 +39,6 @@ class Act:
         self.buf = buf if buf is not None else torch.empty(pad + T, H, W, C, device=device, dtype=torch.bfloat16)
         self.stats = None     # (partial sums tensor, slots) written by the producing conv's epilogue
 
-    def without_halo(self):
-        return self if self.pad == 0 else Act(self.T, self.H, self.W, self.C, 0, None, buf=self.body)
-
     @property
     def frame_elems(self):
         return self.H * self.W * self.C
@@ -74,8 +71,8 @@ class B200VideoVAE(EngineModule):
         self.debug = None           # set by apply_model_specific_config (model_configuration.py:1270-1272)
         self.tensor_offload_device = None
         # encode / decode sequenced by the native runtime (csrc/vae_engine.cu; default) or by this module's Python
-        # methods (per-call profiling, A/B)
-        self.native = os.environ.get("SVR2_NATIVE_VAE", "1") != "0"
+        # methods (per-call profiling, tests against the native runtime)
+        self.native = True
         self._ws_bytes: Dict[tuple, int] = {}
 
     # ---- native runtime (csrc/vae_engine.cu): the same sequences in C++ on a svr2_t handle -------------------
@@ -135,7 +132,7 @@ class B200VideoVAE(EngineModule):
         return self._ws_bytes[key]
 
     def _use_native(self) -> bool:
-        return self.native and lib.PROFILER is None and self.fuse_shortcut and self.single_pass_attention
+        return self.native and lib.PROFILER is None
 
     def _free_bytes(self) -> int:
         """Free HBM incl. torch's cached blocks and the engine's resident workspace (it is regrown on demand)."""
@@ -237,8 +234,6 @@ class B200VideoVAE(EngineModule):
             W[p + "conv2+shortcut.weight"] = torch.cat([W[p + "conv2.weight"], wsc], 1).contiguous()
             W[p + "conv2+shortcut.bias"] = (W[p + "conv2.bias"].float() + W[p + "conv_shortcut.bias"].float()
                                             ).to(torch.bfloat16).contiguous()
-        self.fuse_shortcut = os.environ.get("SVR2_FUSE_SHORTCUT", "1") != "0"      # 0: separate launch (A/B measurements)
-        self.single_pass_attention = os.environ.get("SVR2_VAE_ATTN", "single") != "two_pass"   # two_pass: exact path only
         self.W = self._register("w", W)
 
     # ---- temporal slicing state -------------------------------------------
@@ -280,11 +275,9 @@ class B200VideoVAE(EngineModule):
         return y
 
     def _conv(self, x: Act, prefix: str, *, out_pad=0, residual: Optional[Act] = None, stride_t=1, stride_hw=1,
-              cout=None, cin=None, stats=False) -> Act:
+              stats=False) -> Act:
         w = self.W[prefix + ".weight"]
         kt, kh, kw = self.meta[prefix + ".weight.k"]
-        Cout = cout if cout is not None else w.shape[0]
-        Cin = cin if cin is not None else x.C
         assert x.pad == kt - 1, f"{prefix}: conv with kt={kt} needs a {kt - 1}-frame halo, got {x.pad}"
         x_ptr, T_in_total = lib.ptr(x.buf), x.pad + x.T
         if stride_t == 2 and not self._first:
@@ -304,7 +297,7 @@ class B200VideoVAE(EngineModule):
             res_ptr = c_void_p(residual.body_ptr() - out_pad * y.frame_elems * 2)
         epi = lib.EPI_BIAS | (lib.EPI_RESIDUAL if residual is not None else 0)
         pad_hw = 1 if (stride_hw == 1 and kh == 3) else 0
-        args = (x_ptr, T_in_total, x.H, x.W, Cin, lib.ptr(w), w.shape[0], kt, kh, kw, stride_t, stride_hw,
+        args = (x_ptr, T_in_total, x.H, x.W, x.C, lib.ptr(w), w.shape[0], kt, kh, kw, stride_t, stride_hw,
                 pad_hw, T_out, epi, lib.ptr(self.W[prefix + ".bias"]), res_ptr, lib.ptr(y.buf), out_pad,
                 int(out_pad > 0 and self._first), w.shape[0])
         name, extra = "svr2_conv3d_bf16", ()
@@ -317,7 +310,7 @@ class B200VideoVAE(EngineModule):
         lib.call(name, *args, *extra, lib.stream(),
                  flops=2.0 * T_out * Ho * Wo * self.meta[prefix + ".weight.real"][0] * kt * kh * kw
                  * self.meta[prefix + ".weight.real"][1],
-                 tag=(f"|{Cin}>{w.shape[0]}|k{kt}{kh}{kw}|s{stride_t}{stride_hw}|{T_out}x{Ho}x{Wo}"
+                 tag=(f"|{x.C}>{w.shape[0]}|k{kt}{kh}{kw}|s{stride_t}{stride_hw}|{T_out}x{Ho}x{Wo}"
                       if (lib.PROFILER is not None and lib.PROFILER.detail) else ""))
         self._halo(y, prefix + ":out")
         return y
@@ -328,12 +321,8 @@ class B200VideoVAE(EngineModule):
         h = self._conv(h, p + "conv1", stats=True)
         h = self._gn(h, p + "norm2", True, 2)
         if (p + "conv_shortcut.weight") in self.W:
-            if self.fuse_shortcut:
-                return self._conv_shortcut(h, x, p, out_pad)
-            sc = self._conv(x.without_halo(), p + "conv_shortcut")
-        else:
-            sc = x
-        return self._conv(h, p + "conv2", out_pad=out_pad, residual=sc, stats=True)
+            return self._conv_shortcut(h, x, p, out_pad)
+        return self._conv(h, p + "conv2", out_pad=out_pad, residual=x, stats=True)
 
     def _conv_shortcut(self, h: Act, x: Act, p: str, out_pad: int) -> Act:
         """conv2(h) + conv_shortcut(x) as one implicit GEMM over [h ; x] (see _load); statistics for the next GroupNorm."""
@@ -355,9 +344,9 @@ class B200VideoVAE(EngineModule):
         self._halo(y, p + "conv2:out")
         return y
 
-    def _attention(self, x: Act, p: str) -> Act:
+    def _attention(self, x: Act, p: str, single_pass: bool = True) -> Act:
         """UNetMidBlock3D per-frame attention (attn_video_vae.py:656-668): GN -> q,k,v -> 1-head
-        softmax(q k^T / sqrt(C)) v -> out proj -> + x."""
+        softmax(q k^T / sqrt(C)) v -> out proj -> + x.  ``single_pass=False`` runs only the exact two-pass launches."""
         C, n = x.C, x.H * x.W
         dev = self.device
         y = self._gn(x, p + "group_norm", False, 0)
@@ -391,7 +380,7 @@ class B200VideoVAE(EngineModule):
         # by the row sum in its epilogue.  Exact (softmax is shift-invariant; bf16 rounding is relative) as long as the
         # true row maximum is within 2^96 of the sampled one — checked on the device; the exact two-pass launches below
         # are conditional on that flag and never ran in any test or benchmark.
-        single = self.single_pass_attention and n >= 256 and n % 8 == 0
+        single = single_pass and n >= 256 and n % 8 == 0
         if single:
             k_sub_stride = 16
             n_sub = (n + k_sub_stride - 1) // k_sub_stride

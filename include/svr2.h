@@ -239,8 +239,6 @@ int svr2_linear_ex_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, 
 int svr2_rowstat_max(const void* partial, int slots, int64_t ld, float* mhat, int rows, int* flag_reset, void* stream);
 int svr2_pexp_stat_combine(const void* partial, int slots, int64_t ld, const float* mhat, float* rowscale, int rows,
                            int* flag, void* stream);
-/* row softmax fp32 -> bf16 (materialised-score variant, kept for small problems / tests) */
-int svr2_softmax_rows_bf16(const float* s, int64_t lds, void* p, int64_t ldp, int rows, int cols, void* stream);
 int svr2_transpose_bf16(const void* in, int64_t ld_in, void* out, int64_t ld_out, int rows, int cols, void* stream);
 
 /* layout glue (optimization/performance.py:12-166): NCDHW any-float <-> NDHWC bf16 with halo / channel pad */

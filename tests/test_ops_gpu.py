@@ -338,11 +338,7 @@ def test_groupnorm(svr2lib, C, hw, frames, silu):
     assert torch.equal(y[0], y[2]) and torch.equal(y[1], y[2])
 
 
-def test_softmax_transpose_misc(svr2lib):
-    s = rnd(37, 1000, seed=1) * 3
-    p = torch.empty(37, 1000, device=DEV, dtype=torch.bfloat16)
-    svr2lib.call("svr2_softmax_rows_bf16", svr2lib.ptr(s), 1000, svr2lib.ptr(p), 1000, 37, 1000, svr2lib.stream())
-    assert_close(p, torch.softmax(s, -1), 3e-3, "softmax")
+def test_transpose_misc(svr2lib):
     a = bf(rnd(70, 130, seed=2))
     t = torch.empty(130, 72, device=DEV, dtype=torch.bfloat16)
     svr2lib.call("svr2_transpose_bf16", svr2lib.ptr(a), 130, svr2lib.ptr(t), 72, 70, 130, svr2lib.stream())

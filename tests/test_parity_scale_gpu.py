@@ -9,7 +9,7 @@ bf16 rounding flow ("ref_bf16"); the engine goes through the C ABI.  Stated tole
   on the same inputs (the reference-vs-reference floor is recorded beside it);
 * VAE at 1088 x 1920: >= 40 dB vs fp32 and never more than 3 dB below the reference's bf16 flow (random weights
   amplify bf16 noise; the reference's bf16 flow is the bar);
-* single ops at 4K shapes (band raster, swap-AB, CTA pairs, fused GroupNorm statistics, chunked two-pass attention at
+* single ops at 4K shapes (band raster, swap-AB, fused GroupNorm statistics, chunked two-pass attention at
   n = 129 600, pixel-shuffle store): relative L2 error <= 4e-3 (conv / shuffle), <= 1e-2 (attention) vs torch fp32 on
   bf16-rounded operands;
 * whole clip (pre-process -> encode -> x0.9152 -> DiT -> noise - v -> /0.9152 -> decode -> crop) vs the oracle chain
