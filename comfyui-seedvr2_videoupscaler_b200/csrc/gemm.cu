@@ -8,11 +8,14 @@
 // temporal halo is two real frames stored in front of every activation tensor).
 //
 // Roles (384 threads, 1 CTA / SM, grid = #SMs, static tile schedule):
-//   warps 0,3 : TMA producers (even / odd k-blocks of a kStages-deep smem ring, 128B-swizzled K-major tiles)
-//   warps 1,2 : idle
-//   warps 4-11: two MMA warpgroups (wgmma m64 x BLOCK_N x 16, 64 tile rows each, fp32 accumulators in registers),
-//               then the epilogue (accumulators -> fp32 tile in shared memory over the drained ring -> one row per
-//               thread -> fused math -> swizzled smem slab -> row-contiguous 16-byte global stores)
+//   warps 0,3  : TMA producers (even / odd k-blocks of a kStages-deep smem ring, 128B-swizzled K-major tiles)
+//   warps 4-11 : two MMA warpgroups (wgmma m64 x BLOCK_N x 16, 64 tile rows each, fp32 accumulators in registers)
+//   KIND_BF16  : the MMA warpgroups round bf16(acc + bias) into a dedicated bf16 tile and go on with the next tile's
+//                MMAs; warps 1,2 run the rest of the epilogue from that tile (activation, gate, residual, GroupNorm
+//                partial sums, row-contiguous 16-byte global stores, halo copies) under those MMAs
+//   other kinds: warps 1,2 idle; the MMA warpgroups also run the epilogue (accumulators -> fp32 tile in shared memory
+//                over the drained ring -> one row per thread -> fused math -> swizzled smem slab -> global stores), so
+//                the next tile's loads wait for it
 //
 // Reference semantics replaced: nn.Linear (dit_3b/mmattn.py:56-59,173,269; mlp.py:56-61;
 // patch_v1.py:37,62), InflatedCausalConv3d (causal_inflation_lib.py:213-305), Upsample3D's
@@ -36,7 +39,6 @@ namespace svr2 {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
 constexpr int WGMMA_K = 16;
-constexpr int kNumThreads = 384;   // 4 producer-side warps + 2 MMA / epilogue warpgroups
 
 struct GemmParams {
   int M, N, K;
@@ -102,12 +104,15 @@ enum : int {
   EPI_ROWSCALE = 1024,  // acc *= rowscale[m] first (un-normalised probabilities x V, divided by the row sum)
 };
 
-template <int BLOCK_N>
+// EPI_WG: the epilogue warps' bf16 tile, BLOCK_M x max(BLOCK_N, 32) (swap-AB: 256 pixels x 128 channels);
+// otherwise the per-warp epilogue slabs, 8 warps x (32 rows x 128 B)
+template <int BLOCK_N, bool EPI_WG>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStagingBytes = 8 * 4096;            // epilogue: 8 warps x (32 rows x 128 B)
+  static constexpr int kTileCols = BLOCK_N < 32 ? 32 : BLOCK_N;
+  static constexpr int kStagingBytes = EPI_WG ? BLOCK_M * kTileCols * 2 : 8 * 4096;
   static constexpr int kBudget = 232448 - kStagingBytes - 256 - 1024;   // 227 KB max dynamic smem
   static constexpr int kStages = kBudget / kStageBytes > 8 ? 8 : kBudget / kStageBytes;
   static constexpr int kStagingOffset = kStages * kStageBytes;
@@ -135,6 +140,17 @@ __device__ __forceinline__ void stat_acc(float4& a, const uint4& d) {
     if (e < 2) { a.x += lo + hi; a.y += lo * lo + hi * hi; }
     else { a.z += lo + hi; a.w += lo * lo + hi * hi; }
   }
+}
+
+// bf16(a + b) of 8 bf16 values (the residual add)
+__device__ __forceinline__ uint4 add_bf16x8(const uint4& a, const uint4& b) {
+  const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
+  uint32_t o[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e)
+    o[e] = pack_bf16x2(__uint_as_float(aw[e] << 16) + __uint_as_float(bw[e] << 16),
+                       __uint_as_float(aw[e] & 0xffff0000u) + __uint_as_float(bw[e] & 0xffff0000u));
+  return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 // Conv m-tile raster.  A causal 3x3x3 conv reads every input frame for three consecutive output frames; in
@@ -174,6 +190,17 @@ enum : int { KIND_BF16 = 0, KIND_SWIGLU = 1, KIND_F32 = 2, KIND_ROWSTAT = 3, KIN
              KIND_BF16_RS = 7,
              KIND_PEXP_STAT = 8 };   // KIND_PEXP that also emits per-slot (max score, sum of exponentials)   // KIND_BF16 with a per-row scale on the accumulator (its own instantiation: a runtime test in
                                    // the shared per-element loop cost the pixel-shuffle store 50 %)   // QKV projection + q/k RMSNorm + RoPE (21 / 10 frequencies per axis) + window scatter
+
+// KIND_BF16 epilogues start with bf16(acc + bias), and everything after it acts on that bf16 value: the MMA warpgroups
+// compute it and hand a bf16 tile to the two epilogue warps.  The other kinds need the fp32 accumulators (or a
+// row-wide first step) in the epilogue and keep it on the MMA warpgroups.
+template <int KIND> constexpr bool kEpiWG = KIND == KIND_BF16;
+constexpr int kNumThreads = 384;   // producer warpgroup (2 TMA warps, 2 epilogue warps for KIND_BF16) + 2 MMA warpgroups
+constexpr int kEpiWarps = 2;       // KIND_BF16: warps 1 and 2, 64 tile rows each
+
+// 16-byte chunk swizzle of the swap-AB bf16 tile (rows = pixels, 16 chunks of 8 channels): distinct for 8 consecutive
+// pixels (stmatrix rows) and in different halves of the 8-chunk bank cycle for a pixel pair (the epilogue's reads)
+__device__ __forceinline__ int swap_tile_swz(int pix) { return ((pix & 1) << 2) | ((pix >> 1) & 3); }
 
 // One tile's output row of a thread: destination offset (elements), validity, halo duplication.
 struct RowDest {
@@ -233,17 +260,22 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_a2, const GemmParams p) {
   if (p.run_if != nullptr && *p.run_if == 0) return;     // conditional launch: every thread of every CTA sees the same flag
-  using L = SmemLayout<BLOCK_N>;
+  constexpr bool EPI_WG = kEpiWG<KIND>;
+  static_assert(EPI_WG || (!SWAP && EPI_CT < 0), "swap-AB and compile-time epilogues are KIND_BF16 only");
+  using L = SmemLayout<BLOCK_N, EPI_WG>;
   constexpr int kStages = L::kStages;
   constexpr int ACC_STRIDE = BLOCK_N < 32 ? 32 : BLOCK_N;   // accumulator columns the epilogue addresses
   constexpr int ACC_LD = ACC_STRIDE + 4;                    // fp32 row pitch of the shared accumulator tile
-  static_assert(BLOCK_M * ACC_LD * 4 <= L::kStagingOffset, "the accumulator tile overlays the operand ring");
+  static_assert(EPI_WG || BLOCK_M * ACC_LD * 4 <= L::kStagingOffset, "the accumulator tile overlays the operand ring");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* acc_free = empty_bar + kStages;      // the epilogue is done with the accumulator tile (it overlays the ring)
+  uint64_t* tile_full = acc_free + 1;            // EPI_WG: the MMA warpgroups have written the bf16 tile
+  uint64_t* tile_empty = acc_free + 2;           // EPI_WG: the epilogue warps have read it
   const float* acc_s = reinterpret_cast<const float*>(smem);
+  uint8_t* tile_s = smem + L::kStagingOffset;    // EPI_WG: the bf16 tile
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -258,7 +290,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2);                  // one arrive per consumer warpgroup
     }
-    mbar_init(acc_free, 256);
+    if constexpr (EPI_WG) {
+      mbar_init(tile_full, 256);
+      mbar_init(tile_empty, 32 * kEpiWarps);
+    } else {
+      mbar_init(acc_free, 256);
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -273,8 +310,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // ========================= TMA producers (2 warps) =========================
     // One thread of warp 0 feeds the even k-blocks of the ring, one thread of warp 3 the odd ones, so that the
     // per-k-block issue path (barrier poll, expect-tx, two TMA issues) of one thread never paces the MMAs.
-    // The shared accumulator tile of the epilogue overlays the ring: a tile's loads start once the previous
-    // tile's epilogue has released it (acc_free).
+    // Without the epilogue warps the shared accumulator tile of the epilogue overlays the ring: a tile's loads
+    // start once the previous tile's epilogue has released it (acc_free).
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -296,7 +333,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         if (++stage == kStages) { stage = 0; phase ^= 1; }
       };
       auto tile_start = [&]() {
-        if (it > 0) mbar_wait(acc_free, (it - 1) & 1u);
+        if (!EPI_WG && it > 0) mbar_wait(acc_free, (it - 1) & 1u);
         ++it;
       };
       if (a_mode == 0) {
@@ -366,23 +403,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       }
     }
   } else if (warp >= 4) {
-    // ========================= MMA + epilogue (2 warpgroups) =========================
+    // ========================= MMA warpgroups (2) =========================
     // Mainloop: warpgroup wg owns tile rows [64 wg, 64 wg + 64): one wgmma m64 x BLOCK_N x 16 per 16 columns of K,
     // fp32 accumulators in registers, A and B straight from the 128B-swizzled stages.  The stage of k-block kb is
     // released once the MMAs of kb + 1 are issued and those of kb have retired (one MMA group in flight).
-    // The accumulators then go to a row-major fp32 tile in shared memory (over the drained operand ring), and the
-    // epilogue below reads its rows from there:
-    // Two warps per 32-row quadrant (warp % 4), each owning half of the tile's columns.
-    // Phase 1: a thread owns one accumulator row: 32 columns at a time, fused math, result
-    //          (bf16 or fp32) into a per-warp XOR-swizzled staging slab (32 rows x 128 B).
-    // Phase 2: the warp re-reads the slab row-major so that every global load/store instruction covers
-    //          contiguous 128-byte row segments (16 B per lane); residual loads are issued in batches
-    //          before use, then add + store (+ halo copies).
+    // `tail` then takes the accumulators out of the registers.
     const int wg = (warp - 4) >> 2;
     int mstage = 0;
     uint32_t mphase = 0;
     uint32_t it = 0;
-    auto mainloop = [&]() {
+    auto mainloop = [&](auto&& tail) {
       float d[BLOCK_N / 2];
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
@@ -409,530 +439,623 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       wgmma_wait<0>();
       wgmma_fence_regs(d);
       if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
-      named_bar_sync(1, 256);                    // both warpgroups' MMAs have read their last operands
-      float* acc_w = reinterpret_cast<float*>(smem);
-      const int r0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);
-#pragma unroll
-      for (int i = 0; i < BLOCK_N / 2; i += 4) {
-        const int col = (i >> 2) * 8 + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(acc_w + r0 * ACC_LD + col) = make_float2(d[i], d[i + 1]);
-        *reinterpret_cast<float2*>(acc_w + (r0 + 8) * ACC_LD + col) = make_float2(d[i + 2], d[i + 3]);
-      }
-      named_bar_sync(1, 256);
+      tail(d);
     };
-    constexpr bool IS_BF16 = KIND == KIND_BF16 || KIND == KIND_BF16_RS;
-    constexpr bool IS_PEXP = KIND == KIND_PEXP || KIND == KIND_PEXP_STAT;
-    constexpr int N_COLS = KIND == KIND_SWIGLU ? ACC_STRIDE / 2 : ACC_STRIDE;   // output columns per tile
-    constexpr int COLS_W = N_COLS >= 64 ? N_COLS / 2 : N_COLS;                 // columns per epilogue warp
-    constexpr int PH_COLS = KIND == KIND_F32 ? 32 : (COLS_W < 64 ? COLS_W : 64);
-    constexpr int CPR = KIND == KIND_F32 ? PH_COLS / 4 : PH_COLS / 8;    // 16-byte chunks per staged row
-    constexpr int ROWS_PER_IT = 32 / CPR;
-    constexpr int N_IT = 32 / ROWS_PER_IT;                                // warp-wide accesses per phase
-    constexpr int kBatch = N_IT < 4 ? N_IT : 4;
-    const int q = warp & 3;               // 32-row quadrant of the tile this warp's epilogue covers
-    const int half = (warp - 4) >> 2;     // which half of the columns
-    const int row = q * 32 + lane;        // tile row owned by this thread
-    const bool active = (N_COLS >= 64) || (half == 0);
-    const int col_lo = (N_COLS >= 64) ? half * COLS_W : 0;
-    uint8_t* slab = smem + L::kStagingOffset + (warp - 4) * 4096;
     const int epi = EPI_CT >= 0 ? EPI_CT : p.epi;
-    const int n_lim = KIND == KIND_SWIGLU ? p.N / 2 : p.N;
     const __nv_bfloat16* __restrict__ bias = p.bias;
-    const float* __restrict__ gate = p.gate;
-    const __nv_bfloat16* __restrict__ resid = p.residual;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-      int m_blk, n_blk;
-      tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
-      if (it++ > 0) {                        // the previous tile's epilogue is done with the accumulator tile
-        fence_proxy_async_smem();
-        mbar_arrive(acc_free);
+    if constexpr (EPI_WG) {
+      // bf16(acc + bias) -- the first rounding point of every KIND_BF16 epilogue, the same fp32 add and round to
+      // nearest even -- into the bf16 tile with stmatrix, then on to the next tile.  A warp's fragment is 16 rows:
+      // register group i..i+7 covers columns 16 (i / 8) .. +15, i.e. four 8x8 matrices (rows r0 / r0 + 8, column
+      // halves), lanes 8j..8j+7 address the 16-byte rows of matrix j.  Row-major tile rows, 16-byte chunks XOR-swizzled
+      // by (row % 8): conflict-free for the matrix stores and for the epilogue's 8-lane row reads.  Swap-AB: the rows
+      // are output channels and the epilogue reads pixels, so the matrices are stored transposed into a pixel-major
+      // tile [256 pixels][128 channels].
+      const int r0 = wg * 64 + ((warp & 3) << 4);
+      const uint32_t tbase = smem_u32(tile_s);
+      const int lr = lane & 7, mj = lane >> 3;
+      auto store_tile = [&](float (&d)[BLOCK_N / 2], int n_blk) {
+        if (it > 0) mbar_wait(tile_empty, (it - 1) & 1u);   // the epilogue warps are done with the previous tile
+        if constexpr (SWAP) {
+          const int co = n_blk * BLOCK_M + r0 + (lane >> 2);
+          const bool has_bias = (epi & EPI_BIAS) != 0;
+          const float b0 = (has_bias && co < p.N) ? __bfloat162float(bias[co]) : 0.f;
+          const float b1 = (has_bias && co + 8 < p.N) ? __bfloat162float(bias[co + 8]) : 0.f;
+          const int chunk = (r0 >> 3) + (mj & 1);
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 2; i += 8) {
+            const int pix = (i >> 3) * 16 + ((mj >> 1) << 3) + lr;
+            stmatrix_x4_trans(tbase + pix * 256 + ((chunk ^ swap_tile_swz(pix)) << 4),
+                              pack_bf16x2(d[i] + b0, d[i + 1] + b0), pack_bf16x2(d[i + 2] + b1, d[i + 3] + b1),
+                              pack_bf16x2(d[i + 4] + b0, d[i + 5] + b0), pack_bf16x2(d[i + 6] + b1, d[i + 7] + b1));
+          }
+        } else {
+          constexpr int ROW_B = L::kTileCols * 2;
+          constexpr int SWZ = (L::kTileCols / 8 < 8 ? L::kTileCols / 8 : 8) - 1;
+          const int row = r0 + ((mj & 1) << 3) + lr;
+          const int cn0 = n_blk * BLOCK_N + 2 * (lane & 3);
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 2; i += 8) {
+            float x[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) x[e] = d[i + e];
+            if (epi & EPI_BIAS) {
+              const int cn = cn0 + (i >> 3) * 16;
+              const uint32_t bl = cn < p.N ? __ldg(reinterpret_cast<const unsigned int*>(bias + cn)) : 0u;
+              const uint32_t bh = cn + 8 < p.N ? __ldg(reinterpret_cast<const unsigned int*>(bias + cn + 8)) : 0u;
+              x[0] += __uint_as_float(bl << 16); x[1] += __uint_as_float(bl & 0xffff0000u);
+              x[2] += __uint_as_float(bl << 16); x[3] += __uint_as_float(bl & 0xffff0000u);
+              x[4] += __uint_as_float(bh << 16); x[5] += __uint_as_float(bh & 0xffff0000u);
+              x[6] += __uint_as_float(bh << 16); x[7] += __uint_as_float(bh & 0xffff0000u);
+            }
+            const int chunk = (i >> 3) * 2 + (mj >> 1);
+            stmatrix_x4(tbase + row * ROW_B + ((chunk ^ (row & SWZ)) << 4), pack_bf16x2(x[0], x[1]),
+                        pack_bf16x2(x[2], x[3]), pack_bf16x2(x[4], x[5]), pack_bf16x2(x[6], x[7]));
+          }
+        }
+        mbar_arrive(tile_full);
+      };
+      for (int tile = tile0; tile < num_tiles; tile += tile_step, ++it) {
+        int m_blk, n_blk;
+        tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
+        mainloop([&](float (&d)[BLOCK_N / 2]) { store_tile(d, n_blk); });
       }
-      mainloop();
-      if constexpr (SWAP) {
-        // accumulator lanes = output channels (this thread: co), columns = the tile's 256 pixels.
-        int t_o, th, tw;
-        conv_tile(p, m_blk, t_o, th, tw);
-        const int r = th * p.tiles_w + tw;                        // tile index within the frame (statistics slot)
-        const int h0 = th * p.bh, w0 = tw * p.bw;
-        const int co = n_blk * BLOCK_M + row;
-        const float bsc = ((epi & EPI_BIAS) && co < p.N) ? __bfloat162float(bias[co]) : 0.f;
-        const long long fbase = (long long)(t_o + p.out_t_pad) * p.out_frame_stride + n_blk * BLOCK_M + q * 32;
-        const bool dup_t = p.out_dup_head && t_o == 0;
+    } else {
+      // The accumulators go to a row-major fp32 tile in shared memory (over the drained operand ring), and the
+      // epilogue below reads its rows from there:
+      // Two warps per 32-row quadrant (warp % 4), each owning half of the tile's columns.
+      // Phase 1: a thread owns one accumulator row: 32 columns at a time, fused math, result
+      //          (bf16 or fp32) into a per-warp XOR-swizzled staging slab (32 rows x 128 B).
+      // Phase 2: the warp re-reads the slab row-major so that every global load/store instruction covers
+      //          contiguous 128-byte row segments (16 B per lane); residual loads are issued in batches
+      //          before use, then add + store.
+      auto acc_to_smem = [&](float (&d)[BLOCK_N / 2]) {
+        named_bar_sync(1, 256);                    // both warpgroups' MMAs have read their last operands
+        float* acc_w = reinterpret_cast<float*>(smem);
+        const int r0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; i += 4) {
+          const int col = (i >> 2) * 8 + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(acc_w + r0 * ACC_LD + col) = make_float2(d[i], d[i + 1]);
+          *reinterpret_cast<float2*>(acc_w + (r0 + 8) * ACC_LD + col) = make_float2(d[i + 2], d[i + 3]);
+        }
+        named_bar_sync(1, 256);
+      };
+      constexpr bool IS_BF16 = KIND == KIND_BF16_RS;
+      constexpr bool IS_PEXP = KIND == KIND_PEXP || KIND == KIND_PEXP_STAT;
+      constexpr int N_COLS = KIND == KIND_SWIGLU ? ACC_STRIDE / 2 : ACC_STRIDE;   // output columns per tile
+      constexpr int COLS_W = N_COLS >= 64 ? N_COLS / 2 : N_COLS;                 // columns per epilogue warp
+      constexpr int PH_COLS = KIND == KIND_F32 ? 32 : (COLS_W < 64 ? COLS_W : 64);
+      constexpr int CPR = KIND == KIND_F32 ? PH_COLS / 4 : PH_COLS / 8;    // 16-byte chunks per staged row
+      constexpr int ROWS_PER_IT = 32 / CPR;
+      constexpr int N_IT = 32 / ROWS_PER_IT;                                // warp-wide accesses per phase
+      constexpr int kBatch = N_IT < 4 ? N_IT : 4;
+      const int q = warp & 3;               // 32-row quadrant of the tile this warp's epilogue covers
+      const int half = (warp - 4) >> 2;     // which half of the columns
+      const int row = q * 32 + lane;        // tile row owned by this thread
+      const bool active = (N_COLS >= 64) || (half == 0);
+      const int col_lo = (N_COLS >= 64) ? half * COLS_W : 0;
+      uint8_t* slab = smem + L::kStagingOffset + (warp - 4) * 4096;
+      const int n_lim = KIND == KIND_SWIGLU ? p.N / 2 : p.N;
+      const float* __restrict__ gate = p.gate;
+      const __nv_bfloat16* __restrict__ resid = p.residual;
+      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+        int m_blk, n_blk;
+        tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
+        if (it++ > 0) {                        // the previous tile's epilogue is done with the accumulator tile
+          fence_proxy_async_smem();
+          mbar_arrive(acc_free);
+        }
+        mainloop(acc_to_smem);
+        RowDest dst = row_dest<BLOCK_N>(p, epi, m_blk, n_blk, row, N_COLS);
+        const int n_base = n_blk * (KIND == KIND_SWIGLU ? BLOCK_N / 2 : BLOCK_N);   // first output column
+
+        // Wide path (64-column phases): per-column operands live in lane registers (lane l holds columns 2l, 2l+1
+        // of the phase) and are broadcast by shuffle in phase 1; they are fetched before the accumulator tile is read so
+        // the global-load latency never sits on the epilogue's critical path.
+        constexpr bool kWide = (IS_BF16 || IS_PEXP) && PH_COLS == 64;
+        constexpr int N_PH = kWide ? COLS_W / 64 : 1;
+        uint32_t bias_pk[N_PH];
+        float2 gate2[N_PH];
+        if constexpr (kWide && IS_BF16) {
+#pragma unroll
+          for (int ph = 0; ph < N_PH; ++ph) {
+            const int cn = n_base + col_lo + ph * 64 + 2 * lane;
+            const bool ok = cn < p.N;
+            bias_pk[ph] = ((epi & EPI_BIAS) && ok) ? *reinterpret_cast<const uint32_t*>(bias + cn) : 0u;
+            gate2[ph] = ((epi & EPI_GATE) && ok) ? *reinterpret_cast<const float2*>(gate + cn) : make_float2(0.f, 0.f);
+          }
+        }
+
         const uint32_t t_addr = row * ACC_LD;
-        unsigned short* slab16 = reinterpret_cast<unsigned short*>(slab);
-        float4 st = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 1
-        for (int c0 = half * 128; c0 < half * 128 + 128; c0 += 32) {
-          uint32_t v[32];
-          acc_ld32(acc_s, t_addr + c0, v);
-          // transpose through the slab: row = pixel (128 B stride), 32 channels (64 B) per row
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            slab16[j * 64 + lane] = (unsigned short)(__float_as_uint(bf16_rne(__uint_as_float(v[j]) + bsc)) >> 16);
-          __syncwarp();
-          const int chn = lane & 3, psub = lane >> 2;          // 4 lanes x 16 B per pixel, 8 pixels per access
-          long long off[4];
-          int flags[4];
-          uint4 rv[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int pj = c0 + i * 8 + psub;                  // pixel index within the tile
-            const int ph = pj / p.bw, pw = pj - ph * p.bw;
-            const int h = h0 + ph, w = w0 + pw;
-            const bool ok = (h < p.H_out) && (w < p.W_out) && (n_blk * BLOCK_M + q * 32 + chn * 8 < p.N);
-            off[i] = fbase + ((long long)h * p.W_out + w) * p.ldc + chn * 8;
-            flags[i] = ok ? (dup_t ? 3 : 1) : 0;
-            if ((epi & EPI_RESIDUAL) && ok) rv[i] = *reinterpret_cast<const uint4*>(resid + off[i]);
-          }
-          __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(p.out);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            if (!(flags[i] & 1)) continue;
-            uint4 d = *reinterpret_cast<const uint4*>(slab + (i * 8 + psub) * 128 + chn * 16);
-            if (epi & EPI_RESIDUAL) {
-              const uint32_t dw[4] = {d.x, d.y, d.z, d.w}, rw[4] = {rv[i].x, rv[i].y, rv[i].z, rv[i].w};
-              uint32_t o[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                o[e] = pack_bf16x2(__uint_as_float(dw[e] << 16) + __uint_as_float(rw[e] << 16),
-                                   __uint_as_float(dw[e] & 0xffff0000u) + __uint_as_float(rw[e] & 0xffff0000u));
-              d = make_uint4(o[0], o[1], o[2], o[3]);
-            }
-            *reinterpret_cast<uint4*>(ob + off[i]) = d;
-            if (p.stat_partial) stat_acc(st, d);
-            if (flags[i] & 2) {
-              *reinterpret_cast<uint4*>(ob + off[i] - p.out_frame_stride) = d;
-              *reinterpret_cast<uint4*>(ob + off[i] - 2 * p.out_frame_stride) = d;
-            }
-          }
-          __syncwarp();
-        }
-        if (p.stat_partial) {
-          // lanes with the same channel octet (lane & 3) hold different pixels: fixed-order xor tree
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            st.x += __shfl_xor_sync(0xffffffffu, st.x, o); st.y += __shfl_xor_sync(0xffffffffu, st.y, o);
-            st.z += __shfl_xor_sync(0xffffffffu, st.z, o); st.w += __shfl_xor_sync(0xffffffffu, st.w, o);
-          }
-          if (lane < 4 && t_o < p.T_out) {
-            const int octet = (n_blk * BLOCK_M + q * 32) / 8 + lane;
-            if (octet * 8 < p.N)
-              p.stat_partial[((long long)t_o * p.stat_slots + r * 2 + half) * (p.N / 8) + octet] = st;
-          }
-        }
-        continue;
-      }
-      RowDest dst = row_dest<BLOCK_N>(p, epi, m_blk, n_blk, row, N_COLS);
-      const int n_base = n_blk * (KIND == KIND_SWIGLU ? BLOCK_N / 2 : BLOCK_N);   // first output column
 
-      // Wide path (64-column phases): per-column operands live in lane registers (lane l holds columns 2l, 2l+1
-      // of the phase) and are broadcast by shuffle in phase 1; they are fetched before the accumulator tile is read so
-      // the global-load latency never sits on the epilogue's critical path.
-      constexpr bool kWide = (IS_BF16 || IS_PEXP) && PH_COLS == 64;
-      constexpr int N_PH = kWide ? COLS_W / 64 : 1;
-      uint32_t bias_pk[N_PH];
-      float2 gate2[N_PH];
-      if constexpr (kWide && IS_BF16) {
-#pragma unroll
-        for (int ph = 0; ph < N_PH; ++ph) {
-          const int cn = n_base + col_lo + ph * 64 + 2 * lane;
-          const bool ok = cn < p.N;
-          bias_pk[ph] = ((epi & EPI_BIAS) && ok) ? *reinterpret_cast<const uint32_t*>(bias + cn) : 0u;
-          gate2[ph] = ((epi & EPI_GATE) && ok) ? *reinterpret_cast<const float2*>(gate + cn) : make_float2(0.f, 0.f);
+        float row_lse = 0.f;
+        float2 st_a = make_float2(0.f, 0.f), st_b = make_float2(0.f, 0.f);   // KIND_PEXP_STAT: this thread's row sum
+        if constexpr (IS_PEXP) {
+          const int m = m_blk * BLOCK_M + row;
+          row_lse = (m < p.M) ? gate[m] : 0.f;
         }
-      }
-
-      const uint32_t t_addr = row * ACC_LD;
-
-      float row_lse = 0.f;
-      float2 st_a = make_float2(0.f, 0.f), st_b = make_float2(0.f, 0.f);   // KIND_PEXP_STAT: this thread's row sum
-      if constexpr (IS_PEXP) {
-        const int m = m_blk * BLOCK_M + row;
-        row_lse = (m < p.M) ? gate[m] : 0.f;
-      }
-      float row_scale = 1.f;
-      if constexpr (KIND == KIND_BF16_RS) {
-        const int m = m_blk * BLOCK_M + row;
-        row_scale = (p.a_mode == 0 && m < p.M) ? p.rowscale[m] : 1.f;
-      }
-      if constexpr (KIND == KIND_QKV21 || KIND == KIND_QKV10) {
-        // NaSwinAttention between the QKV projection and the attention call (mmattn.py:199-248, rope.py:116-176), in
-        // the epilogue: a 256-column tile is two heads of q, of k or of v, so this warp's 128 columns are ONE head of
-        // ONE row per thread — per-head RMSNorm is a thread-local sum, RoPE pairs are adjacent registers.  The bf16
-        // rounding of the projection output comes first (the reference normalises the bf16 Linear output in fp32).
-        static_assert(BLOCK_N == 256, "QKV epilogue needs 256-column tiles");
-        constexpr int NF = KIND == KIND_QKV21 ? 21 : 10;
-        const int tpw = p.qkv_inner / 256;               // n-tiles per q / k / v
-        const int which = n_blk / tpw;                   // 0 q, 1 k, 2 v
-        const int m = m_blk * BLOCK_M + row;
-        const bool rvalid = (m < p.M);
-        uint32_t pk[64];
-#pragma unroll
-        for (int c0 = 0; c0 < 128; c0 += 64) {
-          uint32_t v0[32], v1[32];
-          acc_ld32(acc_s, t_addr + col_lo + c0, v0);
-          acc_ld32(acc_s, t_addr + col_lo + c0 + 32, v1);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            pk[c0 / 2 + i] = pack_bf16x2(__uint_as_float(v0[2 * i]), __uint_as_float(v0[2 * i + 1]));
-            pk[c0 / 2 + 16 + i] = pack_bf16x2(__uint_as_float(v1[2 * i]), __uint_as_float(v1[2 * i + 1]));
-          }
+        float row_scale = 1.f;
+        if constexpr (KIND == KIND_BF16_RS) {
+          const int m = m_blk * BLOCK_M + row;
+          row_scale = (p.a_mode == 0 && m < p.M) ? p.rowscale[m] : 1.f;
         }
-        if (which < 2) {
-          float ss = 0.f;
+        if constexpr (KIND == KIND_QKV21 || KIND == KIND_QKV10) {
+          // NaSwinAttention between the QKV projection and the attention call (mmattn.py:199-248, rope.py:116-176), in
+          // the epilogue: a 256-column tile is two heads of q, of k or of v, so this warp's 128 columns are ONE head of
+          // ONE row per thread — per-head RMSNorm is a thread-local sum, RoPE pairs are adjacent registers.  The bf16
+          // rounding of the projection output comes first (the reference normalises the bf16 Linear output in fp32).
+          static_assert(BLOCK_N == 256, "QKV epilogue needs 256-column tiles");
+          constexpr int NF = KIND == KIND_QKV21 ? 21 : 10;
+          const int tpw = p.qkv_inner / 256;               // n-tiles per q / k / v
+          const int which = n_blk / tpw;                   // 0 q, 1 k, 2 v
+          const int m = m_blk * BLOCK_M + row;
+          const bool rvalid = (m < p.M);
+          uint32_t pk[64];
 #pragma unroll
-          for (int i = 0; i < 64; ++i) {
-            const float lo = __uint_as_float(pk[i] << 16), hi = __uint_as_float(pk[i] & 0xffff0000u);
-            ss = fmaf(lo, lo, ss);
-            ss = fmaf(hi, hi, ss);
-          }
-          const float rr = 1.0f / sqrtf(ss * (1.0f / 128.0f) + p.qk_eps);
-          const float2* wn = reinterpret_cast<const float2*>(p.qk_weight + which * 128);
-          int ri[3] = {-1, -1, -1};
-          if (rvalid) {
-            ri[0] = p.tok_rope[(long long)m * 3 + 0];
-            ri[1] = p.tok_rope[(long long)m * 3 + 1];
-            ri[2] = p.tok_rope[(long long)m * 3 + 2];
-          }
-#pragma unroll
-          for (int i = 0; i < 64; ++i) {
-            const float2 w2 = __ldg(wn + i);
-            const float x0 = __uint_as_float(pk[i] << 16) * rr * w2.x;
-            const float x1 = __uint_as_float(pk[i] & 0xffff0000u) * rr * w2.y;
-            float y0 = x0, y1 = x1;
-            if (i < 3 * NF) {                        // compile-time: pairs 3*NF..63 are not rotated
-              const int tr = ri[i / NF];
-              if (tr >= 0) {
-                const float c = __ldg(p.rope_cos + tr * NF + (i % NF)), sn = __ldg(p.rope_sin + tr * NF + (i % NF));
-                y0 = x0 * c - x1 * sn;               // interleaved pairs: (x0, x1) -> (x0 c - x1 s, x1 c + x0 s)
-                y1 = x1 * c + x0 * sn;
-              }
-            }
-            pk[i] = pack_bf16x2(y0, y1);
-          }
-        }
-        __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(which == 0 ? p.out : (which == 1 ? p.out2 : p.out3));
-        const long long roff = rvalid ? (long long)p.tok_dst[m] * p.qkv_inner + (long long)(n_blk - which * tpw) * 256 : 0;
-#pragma unroll
-        for (int ph = 0; ph < 2; ++ph) {
-#pragma unroll
-          for (int c = 0; c < 8; ++c)
-            *reinterpret_cast<uint4*>(slab + lane * 128 + ((c ^ (lane & 7)) << 4)) =
-                make_uint4(pk[ph * 32 + 4 * c], pk[ph * 32 + 4 * c + 1], pk[ph * 32 + 4 * c + 2], pk[ph * 32 + 4 * c + 3]);
-          __syncwarp();
-          const int ch = lane & 7, rsub = lane >> 3;       // 8 x 16-byte chunks per staged row, 4 rows per access
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int r = it * 4 + rsub;
-            const long long off = __shfl_sync(0xffffffffu, roff, r);
-            const int ok = __shfl_sync(0xffffffffu, (int)rvalid, r);
-            if (ok) {
-              const uint4 d = *reinterpret_cast<const uint4*>(slab + r * 128 + ((ch ^ (r & 7)) << 4));
-              *reinterpret_cast<uint4*>(ob + off + col_lo + ph * 64 + ch * 8) = d;
-            }
-          }
-          __syncwarp();
-        }
-      } else if constexpr (KIND == KIND_ROWSTAT) {
-        // attention pass 1: thread-local online (max, sum exp2) over this warp's columns; no staging
-        float mx = -INFINITY, sum = 0.f;
-        if (active) {
-          const float sc = p.out_scale;
-          constexpr int RS = COLS_W >= 64 ? 64 : 32;      // columns in flight per step
-#pragma unroll 1
-          for (int c0 = col_lo; c0 < col_lo + COLS_W; c0 += RS) {
-            uint32_t v[RS];
-            acc_ld32(acc_s, t_addr + c0, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-            if constexpr (RS == 64) acc_ld32(acc_s, t_addr + c0 + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-            const int n0 = n_base + c0;
-            if (sc > 0.f && n0 + RS <= p.N) {
-              // interior step: max on the raw accumulators, the scale folded into the exponent's FMA
-              float cm = __uint_as_float(v[0]);
-#pragma unroll
-              for (int j = 1; j < RS; ++j) cm = fmaxf(cm, __uint_as_float(v[j]));
-              const float m_new = fmaxf(mx, cm * sc);
-              float cs0 = 0.f, cs1 = 0.f;
-#pragma unroll
-              for (int j = 0; j < RS; j += 2) {
-                cs0 += exp2_approx(fmaf(__uint_as_float(v[j]), sc, -m_new));
-                cs1 += exp2_approx(fmaf(__uint_as_float(v[j + 1]), sc, -m_new));
-              }
-              sum = sum * exp2_approx(mx - m_new) + (cs0 + cs1);
-              mx = m_new;
-            } else {
-              float cm = -INFINITY;
-#pragma unroll
-              for (int j = 0; j < RS; ++j) {
-                const float t = (n0 + j < p.N) ? __uint_as_float(v[j]) * sc : -INFINITY;
-                v[j] = __float_as_uint(t);
-                cm = fmaxf(cm, t);
-              }
-              const float m_new = fmaxf(mx, cm);
-              if (m_new > -INFINITY) {
-                float cs = 0.f;
-#pragma unroll
-                for (int j = 0; j < RS; ++j) cs += exp2_approx(__uint_as_float(v[j]) - m_new);
-                sum = sum * exp2_approx(mx - m_new) + cs;
-                mx = m_new;
-              }
-            }
-          }
-        }
-        const int m = m_blk * BLOCK_M + row;
-        if (active && m < p.M) {
-          const int slot = (N_COLS >= 64) ? n_blk * 2 + half : n_blk;
-          reinterpret_cast<float2*>(p.out)[(long long)m * p.ldc + slot] = make_float2(mx, sum);
-        }
-      } else if (active) {
-#pragma unroll 1
-        for (int ph0 = col_lo; ph0 < col_lo + COLS_W; ph0 += PH_COLS) {
-          // ---------------- phase 1 ----------------
-          if constexpr (kWide) {
-            // both 32-column accumulator chunks of the phase loaded at once; every bf16 rounding point is one
-            // cvt.rn.bf16x2 on a column pair (identical to bf16_rne, half the instructions), and the packed
-            // pair is what gets staged
+          for (int c0 = 0; c0 < 128; c0 += 64) {
             uint32_t v0[32], v1[32];
-            acc_ld32(acc_s, t_addr + ph0, v0);
-            acc_ld32(acc_s, t_addr + ph0 + 32, v1);
-            const int phi = (ph0 - col_lo) / 64;
-            uint32_t pk[32];
-            const float sc = p.out_scale;
-            constexpr bool want_stats = KIND == KIND_PEXP_STAT;
-            const bool stats_full = n_base + ph0 + 64 <= p.N;
-            const bool plain = !(epi & (EPI_GELU | EPI_SILU | EPI_GATE));
-            auto elements = [&](auto ragged) {
+            acc_ld32(acc_s, t_addr + col_lo + c0, v0);
+            acc_ld32(acc_s, t_addr + col_lo + c0 + 32, v1);
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              float a = __uint_as_float(i < 16 ? v0[2 * (i & 15)] : v1[2 * (i & 15)]);
-              float b = __uint_as_float(i < 16 ? v0[2 * (i & 15) + 1] : v1[2 * (i & 15) + 1]);
-              if constexpr (IS_PEXP) {
-                // two of every five column pairs take their exp2 on the FMA pipe: the epilogue is MUFU-bound (128 ex2 per
-                // thread and tile = 2048 SM cycles against 1024 of MMA at K = 512)
-                const bool kPoly = (KIND == KIND_PEXP_STAT) && ((i % 5 == 1) || (i % 5 == 3));   // folds after unrolling
-                const float xa = fmaf(a, sc, -row_lse), xb = fmaf(b, sc, -row_lse);
-                const float ea = kPoly ? exp2_poly(xa) : exp2_approx(xa), eb = kPoly ? exp2_poly(xb) : exp2_approx(xb);
-                pk[i] = pack_bf16x2(ea, eb);
-                if constexpr (want_stats) {         // fp32 row sum of the exponentials (two packed chains)
-                  if constexpr (decltype(ragged)::value) {   // last n-tile: zero-padded operand columns are not scores
-                    const int cn = n_base + ph0 + 2 * i;
-                    if (cn < p.N) st_a.x += ea;
-                    if (cn + 1 < p.N) st_a.y += eb;
-                  } else {
-                    if (i & 1) st_b = fadd2(st_b, make_float2(ea, eb));
-                    else st_a = fadd2(st_a, make_float2(ea, eb));
-                  }
-                }
-              } else {
-                if constexpr (KIND == KIND_BF16_RS) {
-                  a *= row_scale;
-                  b *= row_scale;
-                }
-                if (epi & EPI_BIAS) {
-                  const uint32_t bw_ = __shfl_sync(0xffffffffu, bias_pk[phi], i);
-                  a += __uint_as_float(bw_ << 16);
-                  b += __uint_as_float(bw_ & 0xffff0000u);
-                }
-                uint32_t r = pack_bf16x2(a, b);
-                if (!plain) {
-                  if (epi & EPI_GELU) {
-                    r = pack_bf16x2(gelu_tanh_fast(__uint_as_float(r << 16)), gelu_tanh_fast(__uint_as_float(r & 0xffff0000u)));
-                  }
-                  if (epi & EPI_SILU) {
-                    r = pack_bf16x2(silu_fast(__uint_as_float(r << 16)), silu_fast(__uint_as_float(r & 0xffff0000u)));
-                  }
-                  if (epi & EPI_GATE) {
-                    const float g0 = __shfl_sync(0xffffffffu, gate2[phi].x, i);
-                    const float g1 = __shfl_sync(0xffffffffu, gate2[phi].y, i);
-                    r = pack_bf16x2(__uint_as_float(r << 16) * g0, __uint_as_float(r & 0xffff0000u) * g1);
-                  }
-                }
-                pk[i] = r;
-              }
+            for (int i = 0; i < 16; ++i) {
+              pk[c0 / 2 + i] = pack_bf16x2(__uint_as_float(v0[2 * i]), __uint_as_float(v0[2 * i + 1]));
+              pk[c0 / 2 + 16 + i] = pack_bf16x2(__uint_as_float(v1[2 * i]), __uint_as_float(v1[2 * i + 1]));
             }
-            };
-            if (want_stats && !stats_full) elements(std::true_type{});
-            else elements(std::false_type{});
+          }
+          if (which < 2) {
+            float ss = 0.f;
+#pragma unroll
+            for (int i = 0; i < 64; ++i) {
+              const float lo = __uint_as_float(pk[i] << 16), hi = __uint_as_float(pk[i] & 0xffff0000u);
+              ss = fmaf(lo, lo, ss);
+              ss = fmaf(hi, hi, ss);
+            }
+            const float rr = 1.0f / sqrtf(ss * (1.0f / 128.0f) + p.qk_eps);
+            const float2* wn = reinterpret_cast<const float2*>(p.qk_weight + which * 128);
+            int ri[3] = {-1, -1, -1};
+            if (rvalid) {
+              ri[0] = p.tok_rope[(long long)m * 3 + 0];
+              ri[1] = p.tok_rope[(long long)m * 3 + 1];
+              ri[2] = p.tok_rope[(long long)m * 3 + 2];
+            }
+#pragma unroll
+            for (int i = 0; i < 64; ++i) {
+              const float2 w2 = __ldg(wn + i);
+              const float x0 = __uint_as_float(pk[i] << 16) * rr * w2.x;
+              const float x1 = __uint_as_float(pk[i] & 0xffff0000u) * rr * w2.y;
+              float y0 = x0, y1 = x1;
+              if (i < 3 * NF) {                        // compile-time: pairs 3*NF..63 are not rotated
+                const int tr = ri[i / NF];
+                if (tr >= 0) {
+                  const float c = __ldg(p.rope_cos + tr * NF + (i % NF)), sn = __ldg(p.rope_sin + tr * NF + (i % NF));
+                  y0 = x0 * c - x1 * sn;               // interleaved pairs: (x0, x1) -> (x0 c - x1 s, x1 c + x0 s)
+                  y1 = x1 * c + x0 * sn;
+                }
+              }
+              pk[i] = pack_bf16x2(y0, y1);
+            }
+          }
+          __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(which == 0 ? p.out : (which == 1 ? p.out2 : p.out3));
+          const long long roff = rvalid ? (long long)p.tok_dst[m] * p.qkv_inner + (long long)(n_blk - which * tpw) * 256 : 0;
+#pragma unroll
+          for (int ph = 0; ph < 2; ++ph) {
 #pragma unroll
             for (int c = 0; c < 8; ++c)
               *reinterpret_cast<uint4*>(slab + lane * 128 + ((c ^ (lane & 7)) << 4)) =
-                  make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
-          } else {
-#pragma unroll 1
-          for (int c0 = ph0; c0 < ph0 + PH_COLS; c0 += 32) {
-            uint32_t v[32];
-            acc_ld32(acc_s, t_addr + c0, v);
-            const int n0 = n_base + c0;
-            if constexpr (KIND == KIND_SWIGLU) {
-              uint32_t u[32];
-              acc_ld32(acc_s, t_addr + ACC_STRIDE / 2 + c0, u);
-              // rounding points of the reference's bf16 flow (gate, in, silu(gate), product), one
-              // cvt.rn.bf16x2 per column pair each; v[0..15] end up holding the packed output pairs
+                  make_uint4(pk[ph * 32 + 4 * c], pk[ph * 32 + 4 * c + 1], pk[ph * 32 + 4 * c + 2], pk[ph * 32 + 4 * c + 3]);
+            __syncwarp();
+            const int ch = lane & 7, rsub = lane >> 3;       // 8 x 16-byte chunks per staged row, 4 rows per access
 #pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const uint32_t rg = pack_bf16x2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
-                const uint32_t ru = pack_bf16x2(__uint_as_float(u[2 * i]), __uint_as_float(u[2 * i + 1]));
-                const uint32_t rs = pack_bf16x2(silu_fast(__uint_as_float(rg << 16)),
-                                                silu_fast(__uint_as_float(rg & 0xffff0000u)));
-                v[i] = pack_bf16x2(__uint_as_float(rs << 16) * __uint_as_float(ru << 16),
-                                   __uint_as_float(rs & 0xffff0000u) * __uint_as_float(ru & 0xffff0000u));
-              }
-            } else if constexpr (KIND == KIND_F32) {
-              const float sc = p.out_scale;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * sc);
-            } else if constexpr (IS_PEXP) {
-              const float sc = p.out_scale;
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                v[j] = __float_as_uint(bf16_rne(exp2_approx(__uint_as_float(v[j]) * sc - row_lse)));
-            } else {
-              // per-column operands, 8 columns at a time (N % 8 == 0: a group is all-valid or all-OOB)
-#pragma unroll
-              for (int g8 = 0; g8 < 4; ++g8) {
-                const bool ok = (n0 + 8 * g8) < p.N;
-                if (epi & EPI_BIAS) {
-                  const uint4 bv = ok ? *reinterpret_cast<const uint4*>(bias + n0 + 8 * g8) : make_uint4(0, 0, 0, 0);
-                  const uint32_t bw_[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    v[8 * g8 + 2 * e] = __float_as_uint(__uint_as_float(v[8 * g8 + 2 * e]) + __uint_as_float(bw_[e] << 16));
-                    v[8 * g8 + 2 * e + 1] =
-                        __float_as_uint(__uint_as_float(v[8 * g8 + 2 * e + 1]) + __uint_as_float(bw_[e] & 0xffff0000u));
-                  }
-                }
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[8 * g8 + e] = __float_as_uint(bf16_rne(__uint_as_float(v[8 * g8 + e])));
-                if (epi & EPI_GELU) {
-#pragma unroll
-                  for (int e = 0; e < 8; ++e)
-                    v[8 * g8 + e] = __float_as_uint(bf16_rne(gelu_tanh_fast(__uint_as_float(v[8 * g8 + e]))));
-                }
-                if (epi & EPI_SILU) {
-#pragma unroll
-                  for (int e = 0; e < 8; ++e)
-                    v[8 * g8 + e] = __float_as_uint(bf16_rne(silu_fast(__uint_as_float(v[8 * g8 + e]))));
-                }
-                if (epi & EPI_GATE) {
-                  const float4 ga = ok ? *reinterpret_cast<const float4*>(gate + n0 + 8 * g8) : make_float4(0, 0, 0, 0);
-                  const float4 gb = ok ? *reinterpret_cast<const float4*>(gate + n0 + 8 * g8 + 4) : make_float4(0, 0, 0, 0);
-                  const float gg[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
-#pragma unroll
-                  for (int e = 0; e < 8; ++e)
-                    v[8 * g8 + e] = __float_as_uint(bf16_rne(__uint_as_float(v[8 * g8 + e]) * gg[e]));
-                }
+            for (int it = 0; it < 8; ++it) {
+              const int r = it * 4 + rsub;
+              const long long off = __shfl_sync(0xffffffffu, roff, r);
+              const int ok = __shfl_sync(0xffffffffu, (int)rvalid, r);
+              if (ok) {
+                const uint4 d = *reinterpret_cast<const uint4*>(slab + r * 128 + ((ch ^ (r & 7)) << 4));
+                *reinterpret_cast<uint4*>(ob + off + col_lo + ph * 64 + ch * 8) = d;
               }
             }
-            // stage: chunk index within the phase row, XOR-swizzled by the row
-            if constexpr (KIND == KIND_F32) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int ch = j ^ (lane & (CPR - 1));
-                *reinterpret_cast<uint4*>(slab + lane * 128 + ch * 16) =
-                    make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-              }
-            } else if constexpr (KIND == KIND_SWIGLU) {
-              const int cbase = (c0 - ph0) / 8;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const int ch = (cbase + j) ^ (lane & (CPR - 1));
-                *reinterpret_cast<uint4*>(slab + lane * 128 + ch * 16) =
-                    make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-              }
-            } else {
-              // values are already bf16-representable: packing is a byte permute (no conversion)
-              const int cbase = (c0 - ph0) / 8;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const int ch = (cbase + j) ^ (lane & (CPR - 1));
-                *reinterpret_cast<uint4*>(slab + lane * 128 + ch * 16) =
-                    make_uint4(__byte_perm(v[8 * j], v[8 * j + 1], 0x7632), __byte_perm(v[8 * j + 2], v[8 * j + 3], 0x7632),
-                               __byte_perm(v[8 * j + 4], v[8 * j + 5], 0x7632), __byte_perm(v[8 * j + 6], v[8 * j + 7], 0x7632));
-              }
-            }
+            __syncwarp();
           }
-          }   // !kWide
-          __syncwarp();
-          // ---------------- phase 2 ----------------
-          const int ch = lane % CPR, rsub = lane / CPR;
-          const int col = ph0 + (KIND == KIND_F32 ? ch * 4 : ch * 8);
-          const bool col_ok = (n_base + col) < n_lim;
-          float4 st = make_float4(0.f, 0.f, 0.f, 0.f);
+        } else if constexpr (KIND == KIND_ROWSTAT) {
+          // attention pass 1: thread-local online (max, sum exp2) over this warp's columns; no staging
+          float mx = -INFINITY, sum = 0.f;
+          if (active) {
+            const float sc = p.out_scale;
+            constexpr int RS = COLS_W >= 64 ? 64 : 32;      // columns in flight per step
 #pragma unroll 1
-          for (int b0 = 0; b0 < N_IT; b0 += kBatch) {
-            long long off[kBatch];
-            int flags[kBatch];
-            uint4 rv[kBatch];
+            for (int c0 = col_lo; c0 < col_lo + COLS_W; c0 += RS) {
+              uint32_t v[RS];
+              acc_ld32(acc_s, t_addr + c0, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
+              if constexpr (RS == 64) acc_ld32(acc_s, t_addr + c0 + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
+              const int n0 = n_base + c0;
+              if (sc > 0.f && n0 + RS <= p.N) {
+                // interior step: max on the raw accumulators, the scale folded into the exponent's FMA
+                float cm = __uint_as_float(v[0]);
 #pragma unroll
-            for (int i = 0; i < kBatch; ++i) {
-              const int r = (b0 + i) * ROWS_PER_IT + rsub;
-              off[i] = __shfl_sync(0xffffffffu, dst.off, r);
-              const int f = __shfl_sync(0xffffffffu, dst.valid | (dst.dup << 1), r);
-              flags[i] = col_ok ? f : 0;
-              if constexpr (IS_BF16) {
-                if ((epi & EPI_RESIDUAL) && (flags[i] & 1)) rv[i] = *reinterpret_cast<const uint4*>(resid + off[i] + col);
-              }
-            }
+                for (int j = 1; j < RS; ++j) cm = fmaxf(cm, __uint_as_float(v[j]));
+                const float m_new = fmaxf(mx, cm * sc);
+                float cs0 = 0.f, cs1 = 0.f;
 #pragma unroll
-            for (int i = 0; i < kBatch; ++i) {
-              if (!(flags[i] & 1)) continue;
-              const int r = (b0 + i) * ROWS_PER_IT + rsub;
-              uint4 d = *reinterpret_cast<const uint4*>(slab + r * 128 + ((ch ^ (r & (CPR - 1))) << 4));
-              if constexpr (KIND == KIND_F32) {
-                *reinterpret_cast<uint4*>(reinterpret_cast<float*>(p.out) + off[i] + col) = d;
+                for (int j = 0; j < RS; j += 2) {
+                  cs0 += exp2_approx(fmaf(__uint_as_float(v[j]), sc, -m_new));
+                  cs1 += exp2_approx(fmaf(__uint_as_float(v[j + 1]), sc, -m_new));
+                }
+                sum = sum * exp2_approx(mx - m_new) + (cs0 + cs1);
+                mx = m_new;
               } else {
-                __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(p.out);
-                if constexpr (IS_BF16) {
-                  if (epi & EPI_RESIDUAL) {
-                    const uint32_t dw[4] = {d.x, d.y, d.z, d.w}, rw[4] = {rv[i].x, rv[i].y, rv[i].z, rv[i].w};
-                    uint32_t o[4];
+                float cm = -INFINITY;
 #pragma unroll
-                    for (int e = 0; e < 4; ++e)
-                      o[e] = pack_bf16x2(__uint_as_float(dw[e] << 16) + __uint_as_float(rw[e] << 16),
-                                         __uint_as_float(dw[e] & 0xffff0000u) + __uint_as_float(rw[e] & 0xffff0000u));
-                    d = make_uint4(o[0], o[1], o[2], o[3]);
+                for (int j = 0; j < RS; ++j) {
+                  const float t = (n0 + j < p.N) ? __uint_as_float(v[j]) * sc : -INFINITY;
+                  v[j] = __float_as_uint(t);
+                  cm = fmaxf(cm, t);
+                }
+                const float m_new = fmaxf(mx, cm);
+                if (m_new > -INFINITY) {
+                  float cs = 0.f;
+#pragma unroll
+                  for (int j = 0; j < RS; ++j) cs += exp2_approx(__uint_as_float(v[j]) - m_new);
+                  sum = sum * exp2_approx(mx - m_new) + cs;
+                  mx = m_new;
+                }
+              }
+            }
+          }
+          const int m = m_blk * BLOCK_M + row;
+          if (active && m < p.M) {
+            const int slot = (N_COLS >= 64) ? n_blk * 2 + half : n_blk;
+            reinterpret_cast<float2*>(p.out)[(long long)m * p.ldc + slot] = make_float2(mx, sum);
+          }
+        } else if (active) {
+#pragma unroll 1
+          for (int ph0 = col_lo; ph0 < col_lo + COLS_W; ph0 += PH_COLS) {
+            // ---------------- phase 1 ----------------
+            if constexpr (kWide) {
+              // both 32-column accumulator chunks of the phase loaded at once; every bf16 rounding point is one
+              // cvt.rn.bf16x2 on a column pair (identical to bf16_rne, half the instructions), and the packed
+              // pair is what gets staged
+              uint32_t v0[32], v1[32];
+              acc_ld32(acc_s, t_addr + ph0, v0);
+              acc_ld32(acc_s, t_addr + ph0 + 32, v1);
+              const int phi = (ph0 - col_lo) / 64;
+              uint32_t pk[32];
+              const float sc = p.out_scale;
+              constexpr bool want_stats = KIND == KIND_PEXP_STAT;
+              const bool stats_full = n_base + ph0 + 64 <= p.N;
+              const bool plain = !(epi & (EPI_GELU | EPI_SILU | EPI_GATE));
+              auto elements = [&](auto ragged) {
+#pragma unroll
+              for (int i = 0; i < 32; ++i) {
+                float a = __uint_as_float(i < 16 ? v0[2 * (i & 15)] : v1[2 * (i & 15)]);
+                float b = __uint_as_float(i < 16 ? v0[2 * (i & 15) + 1] : v1[2 * (i & 15) + 1]);
+                if constexpr (IS_PEXP) {
+                  // two of every five column pairs take their exp2 on the FMA pipe: the epilogue is MUFU-bound (128 ex2 per
+                  // thread and tile = 2048 SM cycles against 1024 of MMA at K = 512)
+                  const bool kPoly = (KIND == KIND_PEXP_STAT) && ((i % 5 == 1) || (i % 5 == 3));   // folds after unrolling
+                  const float xa = fmaf(a, sc, -row_lse), xb = fmaf(b, sc, -row_lse);
+                  const float ea = kPoly ? exp2_poly(xa) : exp2_approx(xa), eb = kPoly ? exp2_poly(xb) : exp2_approx(xb);
+                  pk[i] = pack_bf16x2(ea, eb);
+                  if constexpr (want_stats) {         // fp32 row sum of the exponentials (two packed chains)
+                    if constexpr (decltype(ragged)::value) {   // last n-tile: zero-padded operand columns are not scores
+                      const int cn = n_base + ph0 + 2 * i;
+                      if (cn < p.N) st_a.x += ea;
+                      if (cn + 1 < p.N) st_a.y += eb;
+                    } else {
+                      if (i & 1) st_b = fadd2(st_b, make_float2(ea, eb));
+                      else st_a = fadd2(st_a, make_float2(ea, eb));
+                    }
                   }
-                }
-                *reinterpret_cast<uint4*>(ob + off[i] + col) = d;
-                if constexpr (IS_BF16) {
-                  if (p.stat_partial) stat_acc(st, d);
-                }
-                if (flags[i] & 2) {
-                  *reinterpret_cast<uint4*>(ob + off[i] - p.out_frame_stride + col) = d;
-                  *reinterpret_cast<uint4*>(ob + off[i] - 2 * p.out_frame_stride + col) = d;
+                } else {
+                  if constexpr (KIND == KIND_BF16_RS) {
+                    a *= row_scale;
+                    b *= row_scale;
+                  }
+                  if (epi & EPI_BIAS) {
+                    const uint32_t bw_ = __shfl_sync(0xffffffffu, bias_pk[phi], i);
+                    a += __uint_as_float(bw_ << 16);
+                    b += __uint_as_float(bw_ & 0xffff0000u);
+                  }
+                  uint32_t r = pack_bf16x2(a, b);
+                  if (!plain) {
+                    if (epi & EPI_GELU) {
+                      r = pack_bf16x2(gelu_tanh_fast(__uint_as_float(r << 16)), gelu_tanh_fast(__uint_as_float(r & 0xffff0000u)));
+                    }
+                    if (epi & EPI_SILU) {
+                      r = pack_bf16x2(silu_fast(__uint_as_float(r << 16)), silu_fast(__uint_as_float(r & 0xffff0000u)));
+                    }
+                    if (epi & EPI_GATE) {
+                      const float g0 = __shfl_sync(0xffffffffu, gate2[phi].x, i);
+                      const float g1 = __shfl_sync(0xffffffffu, gate2[phi].y, i);
+                      r = pack_bf16x2(__uint_as_float(r << 16) * g0, __uint_as_float(r & 0xffff0000u) * g1);
+                    }
+                  }
+                  pk[i] = r;
                 }
               }
-            }
-          }
-          if constexpr (IS_BF16) {
-            if (p.stat_partial && p.a_mode != 0) {
-              // lanes with equal (lane % CPR) own the same channel octet for different rows
+              };
+              if (want_stats && !stats_full) elements(std::true_type{});
+              else elements(std::false_type{});
 #pragma unroll
-              for (int o = CPR; o < 32; o <<= 1) {
-                st.x += __shfl_xor_sync(0xffffffffu, st.x, o); st.y += __shfl_xor_sync(0xffffffffu, st.y, o);
-                st.z += __shfl_xor_sync(0xffffffffu, st.z, o); st.w += __shfl_xor_sync(0xffffffffu, st.w, o);
+              for (int c = 0; c < 8; ++c)
+                *reinterpret_cast<uint4*>(slab + lane * 128 + ((c ^ (lane & 7)) << 4)) =
+                    make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
+            } else {
+#pragma unroll 1
+            for (int c0 = ph0; c0 < ph0 + PH_COLS; c0 += 32) {
+              uint32_t v[32];
+              acc_ld32(acc_s, t_addr + c0, v);
+              if constexpr (KIND == KIND_SWIGLU) {
+                uint32_t u[32];
+                acc_ld32(acc_s, t_addr + ACC_STRIDE / 2 + c0, u);
+                // rounding points of the reference's bf16 flow (gate, in, silu(gate), product), one
+                // cvt.rn.bf16x2 per column pair each; v[0..15] end up holding the packed output pairs
+#pragma unroll
+                for (int i = 0; i < 16; ++i) {
+                  const uint32_t rg = pack_bf16x2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
+                  const uint32_t ru = pack_bf16x2(__uint_as_float(u[2 * i]), __uint_as_float(u[2 * i + 1]));
+                  const uint32_t rs = pack_bf16x2(silu_fast(__uint_as_float(rg << 16)),
+                                                  silu_fast(__uint_as_float(rg & 0xffff0000u)));
+                  v[i] = pack_bf16x2(__uint_as_float(rs << 16) * __uint_as_float(ru << 16),
+                                     __uint_as_float(rs & 0xffff0000u) * __uint_as_float(ru & 0xffff0000u));
+                }
+              } else if constexpr (KIND == KIND_F32) {
+                const float sc = p.out_scale;
+#pragma unroll
+                for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * sc);
+              } else {
+                static_assert(IS_PEXP, "the bf16 kinds take the wide path");
+                const float sc = p.out_scale;
+#pragma unroll
+                for (int j = 0; j < 32; ++j)
+                  v[j] = __float_as_uint(bf16_rne(exp2_approx(__uint_as_float(v[j]) * sc - row_lse)));
               }
-              int t_o, th, tw;
-              conv_tile(p, m_blk, t_o, th, tw);
-              const int rt = th * p.tiles_w + tw;
-              if (lane < CPR && col_ok && m_blk < p.num_m_tiles)
-                p.stat_partial[((long long)t_o * p.stat_slots + rt * 4 + q) * (p.N / 8) + (n_base + col) / 8] = st;
+              // stage: chunk index within the phase row, XOR-swizzled by the row
+              if constexpr (KIND == KIND_F32) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                  const int ch = j ^ (lane & (CPR - 1));
+                  *reinterpret_cast<uint4*>(slab + lane * 128 + ch * 16) =
+                      make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                }
+              } else if constexpr (KIND == KIND_SWIGLU) {
+                const int cbase = (c0 - ph0) / 8;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  const int ch = (cbase + j) ^ (lane & (CPR - 1));
+                  *reinterpret_cast<uint4*>(slab + lane * 128 + ch * 16) =
+                      make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                }
+              } else {
+                // values are already bf16-representable: packing is a byte permute (no conversion)
+                const int cbase = (c0 - ph0) / 8;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  const int ch = (cbase + j) ^ (lane & (CPR - 1));
+                  *reinterpret_cast<uint4*>(slab + lane * 128 + ch * 16) =
+                      make_uint4(__byte_perm(v[8 * j], v[8 * j + 1], 0x7632), __byte_perm(v[8 * j + 2], v[8 * j + 3], 0x7632),
+                                 __byte_perm(v[8 * j + 4], v[8 * j + 5], 0x7632), __byte_perm(v[8 * j + 6], v[8 * j + 7], 0x7632));
+                }
+              }
             }
+            }   // !kWide
+            __syncwarp();
+            // ---------------- phase 2 ----------------
+            const int ch = lane % CPR, rsub = lane / CPR;
+            const int col = ph0 + (KIND == KIND_F32 ? ch * 4 : ch * 8);
+            const bool col_ok = (n_base + col) < n_lim;
+#pragma unroll 1
+            for (int b0 = 0; b0 < N_IT; b0 += kBatch) {
+              long long off[kBatch];
+              int flags[kBatch];
+              uint4 rv[kBatch];
+#pragma unroll
+              for (int i = 0; i < kBatch; ++i) {
+                const int r = (b0 + i) * ROWS_PER_IT + rsub;
+                off[i] = __shfl_sync(0xffffffffu, dst.off, r);
+                const int f = __shfl_sync(0xffffffffu, dst.valid | (dst.dup << 1), r);
+                flags[i] = col_ok ? f : 0;
+                if constexpr (IS_BF16) {
+                  if ((epi & EPI_RESIDUAL) && (flags[i] & 1)) rv[i] = *reinterpret_cast<const uint4*>(resid + off[i] + col);
+                }
+              }
+#pragma unroll
+              for (int i = 0; i < kBatch; ++i) {
+                if (!(flags[i] & 1)) continue;
+                const int r = (b0 + i) * ROWS_PER_IT + rsub;
+                uint4 d = *reinterpret_cast<const uint4*>(slab + r * 128 + ((ch ^ (r & (CPR - 1))) << 4));
+                if constexpr (KIND == KIND_F32) {
+                  *reinterpret_cast<uint4*>(reinterpret_cast<float*>(p.out) + off[i] + col) = d;
+                } else {
+                  __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(p.out);
+                  if constexpr (IS_BF16) {
+                    if (epi & EPI_RESIDUAL) d = add_bf16x8(d, rv[i]);
+                  }
+                  *reinterpret_cast<uint4*>(ob + off[i] + col) = d;
+                }
+              }
+            }
+            __syncwarp();
           }
-          __syncwarp();
-        }
-        if constexpr (KIND == KIND_PEXP_STAT) {
-          if (p.stat2) {     // this thread's row over this warp's columns of the tile: (max score, sum of exponentials)
-            const int m = m_blk * BLOCK_M + row;
-            if (m < p.M) {
-              const int slot = (N_COLS >= 64) ? n_blk * 2 + half : n_blk;
-              p.stat2[(long long)m * p.ld_stat + slot] = make_float2(0.f, (st_a.x + st_b.x) + (st_a.y + st_b.y));
+          if constexpr (KIND == KIND_PEXP_STAT) {
+            if (p.stat2) {     // this thread's row over this warp's columns of the tile: (max score, sum of exponentials)
+              const int m = m_blk * BLOCK_M + row;
+              if (m < p.M) {
+                const int slot = (N_COLS >= 64) ? n_blk * 2 + half : n_blk;
+                p.stat2[(long long)m * p.ld_stat + slot] = make_float2(0.f, (st_a.x + st_b.x) + (st_a.y + st_b.y));
+              }
             }
           }
         }
       }
     }
+  } else {
+    if constexpr (EPI_WG) {
+      // ========================= epilogue warps (KIND_BF16: warps 1, 2) =========================
+      // Warp 1 + e owns the 32-row quadrants q = 2 e, 2 e + 1 of the tile; for each, rows [32 q, 32 q + 32) over all
+      // columns, in 64-column phases (32-column phases below 128-column tiles).  Every global load / store instruction covers contiguous row segments, 16 bytes per
+      // lane; residual loads are issued in batches before use.  The GroupNorm partial sums of a phase go to slot
+      // (tile, q), summed in the same order as when two warps split a quadrant's columns.
+      // Swap-AB: quadrant q is output channels [32 q, 32 q + 32) of the tile's 256 pixels, one pixel half (and
+      // statistics slot) after the other.
+      const int q0 = 2 * (warp - 1);
+      const int epi = EPI_CT >= 0 ? EPI_CT : p.epi;
+      const float* __restrict__ gate = p.gate;
+      const __nv_bfloat16* __restrict__ resid = p.residual;
+      __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(p.out);
+      uint32_t it = 0;
+      for (int tile = tile0; tile < num_tiles; tile += tile_step, ++it) {
+        int m_blk, n_blk;
+        tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
+        mbar_wait(tile_full, it & 1u);
+#pragma unroll 1
+        for (int q = q0; q < q0 + 2; ++q) {
+          const int row = q * 32 + lane;
+          if constexpr (SWAP) {
+            int t_o, th, tw;
+            conv_tile(p, m_blk, t_o, th, tw);
+            const int r = th * p.tiles_w + tw;                        // tile index within the frame (statistics slot)
+            const int h0 = th * p.bh, w0 = tw * p.bw;
+            const long long fbase = (long long)(t_o + p.out_t_pad) * p.out_frame_stride + n_blk * BLOCK_M + q * 32;
+            const bool dup_t = p.out_dup_head && t_o == 0;
+            const int chn = lane & 3, psub = lane >> 2;              // 4 lanes x 16 B per pixel, 8 pixels per access
+            const bool ch_ok = n_blk * BLOCK_M + q * 32 + chn * 8 < p.N;
+#pragma unroll 1
+            for (int half = 0; half < 2; ++half) {
+              float4 st = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+              for (int c0 = half * 128; c0 < half * 128 + 128; c0 += 32) {
+                long long off[4];
+                int flags[4];
+                uint4 rv[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                  const int pj = c0 + i * 8 + psub;                  // pixel index within the tile
+                  const int ph = pj / p.bw, pw = pj - ph * p.bw;
+                  const int h = h0 + ph, w = w0 + pw;
+                  const bool ok = (h < p.H_out) && (w < p.W_out) && ch_ok;
+                  off[i] = fbase + ((long long)h * p.W_out + w) * p.ldc + chn * 8;
+                  flags[i] = ok ? (dup_t ? 3 : 1) : 0;
+                  if ((epi & EPI_RESIDUAL) && ok) rv[i] = *reinterpret_cast<const uint4*>(resid + off[i]);
+                }
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                  if (!(flags[i] & 1)) continue;
+                  const int pj = c0 + i * 8 + psub;
+                  uint4 d = *reinterpret_cast<const uint4*>(tile_s + pj * 256 + (((q * 4 + chn) ^ swap_tile_swz(pj)) << 4));
+                  if (epi & EPI_RESIDUAL) d = add_bf16x8(d, rv[i]);
+                  *reinterpret_cast<uint4*>(ob + off[i]) = d;
+                  if (p.stat_partial) stat_acc(st, d);
+                  if (flags[i] & 2) {
+                    *reinterpret_cast<uint4*>(ob + off[i] - p.out_frame_stride) = d;
+                    *reinterpret_cast<uint4*>(ob + off[i] - 2 * p.out_frame_stride) = d;
+                  }
+                }
+              }
+              if (p.stat_partial) {
+                // lanes with the same channel octet (lane & 3) hold different pixels: fixed-order xor tree
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1) {
+                  st.x += __shfl_xor_sync(0xffffffffu, st.x, o); st.y += __shfl_xor_sync(0xffffffffu, st.y, o);
+                  st.z += __shfl_xor_sync(0xffffffffu, st.z, o); st.w += __shfl_xor_sync(0xffffffffu, st.w, o);
+                }
+                if (lane < 4 && t_o < p.T_out) {
+                  const int octet = (n_blk * BLOCK_M + q * 32) / 8 + lane;
+                  if (octet * 8 < p.N)
+                    p.stat_partial[((long long)t_o * p.stat_slots + r * 2 + half) * (p.N / 8) + octet] = st;
+                }
+              }
+            }
+          } else {
+            constexpr int PH_COLS = ACC_STRIDE >= 128 ? 64 : 32;
+            constexpr int CPR = PH_COLS / 8;                         // 16-byte chunks per phase row
+            constexpr int ROWS_PER_IT = 32 / CPR;
+            constexpr int N_IT = 32 / ROWS_PER_IT;                   // warp-wide accesses per phase
+            constexpr int kBatch = N_IT;   // a phase's residual loads all in flight: two warps cover the whole tile
+            constexpr int ROW_B = L::kTileCols * 2;
+            constexpr int SWZ = (L::kTileCols / 8 < 8 ? L::kTileCols / 8 : 8) - 1;
+            const RowDest dst = row_dest<BLOCK_N>(p, epi, m_blk, n_blk, row, ACC_STRIDE);
+            const int n_base = n_blk * BLOCK_N;
+            const int ch = lane % CPR, rsub = lane / CPR;
+            const bool plain = !(epi & (EPI_GELU | EPI_SILU | EPI_GATE));
+            int t_o = 0, rt = 0;
+            if (p.stat_partial && p.a_mode != 0) {
+              int th, tw;
+              conv_tile(p, m_blk, t_o, th, tw);
+              rt = th * p.tiles_w + tw;
+            }
+#pragma unroll 1
+            for (int ph0 = 0; ph0 < ACC_STRIDE; ph0 += PH_COLS) {
+              const int col = ph0 + ch * 8;
+              const bool col_ok = (n_base + col) < p.N;
+              float gg[8];
+              if (epi & EPI_GATE) {
+                const float4 ga = col_ok ? *reinterpret_cast<const float4*>(gate + n_base + col) : make_float4(0, 0, 0, 0);
+                const float4 gb = col_ok ? *reinterpret_cast<const float4*>(gate + n_base + col + 4) : make_float4(0, 0, 0, 0);
+                gg[0] = ga.x; gg[1] = ga.y; gg[2] = ga.z; gg[3] = ga.w;
+                gg[4] = gb.x; gg[5] = gb.y; gg[6] = gb.z; gg[7] = gb.w;
+              }
+              float4 st = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+              for (int b0 = 0; b0 < N_IT; b0 += kBatch) {
+                long long off[kBatch];
+                int flags[kBatch];
+                uint4 rv[kBatch];
+#pragma unroll
+                for (int i = 0; i < kBatch; ++i) {
+                  const int r = (b0 + i) * ROWS_PER_IT + rsub;
+                  off[i] = __shfl_sync(0xffffffffu, dst.off, r);
+                  const int f = __shfl_sync(0xffffffffu, dst.valid | (dst.dup << 1), r);
+                  flags[i] = col_ok ? f : 0;
+                  if ((epi & EPI_RESIDUAL) && (flags[i] & 1)) rv[i] = *reinterpret_cast<const uint4*>(resid + off[i] + col);
+                }
+#pragma unroll
+                for (int i = 0; i < kBatch; ++i) {
+                  if (!(flags[i] & 1)) continue;
+                  const int tr = q * 32 + (b0 + i) * ROWS_PER_IT + rsub;
+                  uint4 d = *reinterpret_cast<const uint4*>(tile_s + tr * ROW_B + (((col >> 3) ^ (tr & SWZ)) << 4));
+                  if (!plain) {
+                    uint32_t w[4] = {d.x, d.y, d.z, d.w};
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                      if (epi & EPI_GELU)
+                        w[e] = pack_bf16x2(gelu_tanh_fast(__uint_as_float(w[e] << 16)),
+                                           gelu_tanh_fast(__uint_as_float(w[e] & 0xffff0000u)));
+                      if (epi & EPI_SILU)
+                        w[e] = pack_bf16x2(silu_fast(__uint_as_float(w[e] << 16)), silu_fast(__uint_as_float(w[e] & 0xffff0000u)));
+                      if (epi & EPI_GATE)
+                        w[e] = pack_bf16x2(__uint_as_float(w[e] << 16) * gg[2 * e],
+                                           __uint_as_float(w[e] & 0xffff0000u) * gg[2 * e + 1]);
+                    }
+                    d = make_uint4(w[0], w[1], w[2], w[3]);
+                  }
+                  if (epi & EPI_RESIDUAL) d = add_bf16x8(d, rv[i]);
+                  *reinterpret_cast<uint4*>(ob + off[i] + col) = d;
+                  if (p.stat_partial) stat_acc(st, d);
+                  if (flags[i] & 2) {
+                    *reinterpret_cast<uint4*>(ob + off[i] - p.out_frame_stride + col) = d;
+                    *reinterpret_cast<uint4*>(ob + off[i] - 2 * p.out_frame_stride + col) = d;
+                  }
+                }
+              }
+              if (p.stat_partial && p.a_mode != 0) {
+                // lanes with equal (lane % CPR) own the same channel octet for different rows
+#pragma unroll
+                for (int o = CPR; o < 32; o <<= 1) {
+                  st.x += __shfl_xor_sync(0xffffffffu, st.x, o); st.y += __shfl_xor_sync(0xffffffffu, st.y, o);
+                  st.z += __shfl_xor_sync(0xffffffffu, st.z, o); st.w += __shfl_xor_sync(0xffffffffu, st.w, o);
+                }
+                if (lane < CPR && col_ok && m_blk < p.num_m_tiles)
+                  p.stat_partial[((long long)t_o * p.stat_slots + rt * 4 + q) * (p.N / 8) + (n_base + col) / 8] = st;
+              }
+            }
+          }
+        }
+        mbar_arrive(tile_empty);
+      }
+    }
   }
-
 }
 
 // ----------------------------------------------------------------------------
@@ -999,7 +1122,7 @@ template <int BLOCK_N, int KIND, bool SWAP = false, int EPI_CT = -1>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p_in, cudaStream_t stream,
                        const CUtensorMap* ta2_opt = nullptr) {
   const CUtensorMap& ta2 = ta2_opt ? *ta2_opt : ta;
-  using L = SmemLayout<BLOCK_N>;
+  using L = SmemLayout<BLOCK_N, kEpiWG<KIND>>;
   auto kern = gemm_wgmma_kernel<BLOCK_N, KIND, SWAP, EPI_CT>;
   GemmParams p = p_in;
   {

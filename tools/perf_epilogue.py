@@ -65,7 +65,8 @@ def mk_up():
                             lib.ptr(y), 2, 1, lib.stream())
 cases.append(("upsample_256 2x1080x1920", mk_up, 2.0 * 2 * 1080 * 1920 * 256 * 1024))
 for nm, Cin, Cout, k3, T, H, W in (("sc256to128", 256, 128, 1, 2, 2160, 3840), ("sc512to256", 512, 256, 1, 4, 1080, 1920),
-                                    ("c256", 256, 256, 3, 2, 1080, 1920), ("c128", 128, 128, 3, 2, 2160, 3840)):
+                                    ("c256", 256, 256, 3, 2, 1080, 1920), ("c128", 128, 128, 3, 2, 2160, 3840),
+                                    ("c512", 512, 512, 3, 2, 540, 960)):   # longest K (13824): 3-stage ring
     def mk(Cin=Cin, Cout=Cout, k3=k3, T=T, H=H, W=W):
         pad = k3 - 1
         x = rnd(T + pad, H, W, Cin); w = rnd(Cout, k3 ** 3 * Cin) * 0.02; b = rnd(Cout)
