@@ -117,6 +117,17 @@ def sample_to_image(sample: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def sample_to_image_rgba(sample: torch.Tensor, image: torch.Tensor) -> torch.Tensor:
+    """``sample_to_image`` into channels 0..2 of an RGBA image ``[T, H, W, 4]`` bf16 whose channel 3 already holds the
+    alpha (``generation_phases.py:1325-1345``: only the RGB is normalised, the alpha is kept as computed)."""
+    x = _as_planes(sample)
+    T, _, H, W = x.shape
+    assert image.shape == (T, H, W, 4) and image.dtype == torch.bfloat16 and image.is_contiguous()
+    lib.call("svr2_sample_to_image_rgba_bf16", lib.ptr(x), lib.ptr(image), T, H * W, lib.stream(),
+             nbytes=4.0 * x.numel())
+    return image
+
+
 def apply_color_correction(sample: torch.Tensor, input_video: torch.Tensor, color_correction: str = "lab",
                            debug=None) -> torch.Tensor:
     """The method switch of ``generation_phases.py:1299-1317``."""

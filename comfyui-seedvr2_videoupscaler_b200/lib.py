@@ -93,6 +93,10 @@ SIGNATURES = {
     "svr2_resize_scratch_bytes": [c_int, c_int, c_int, c_int],
     "svr2_resize_bicubic_aa_bf16": [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P, c_int64,
                                     _P],
+    "svr2_alpha_upscale_scratch_bytes": [c_int, c_int, c_int, c_int, c_int],
+    "svr2_alpha_upscale": [_P, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int64, _P],
+    "svr2_sobel_edges_f32": [_P, c_int, c_int, c_int, _P, _P, c_int64, _P],
+    "svr2_sample_to_image_rgba_bf16": [_P, _P, c_int, c_int64, _P],
 }
 
 _lib = None
@@ -138,7 +142,9 @@ def stream():
 KERNELS_PER_CALL = {"svr2_groupnorm_bf16": 3, "svr2_groupnorm_from_stats_bf16": 2,
                     "svr2_resize_bicubic_aa_bf16": 3,      # two tap-table kernels + the resize
                     "svr2_adain_bf16": 2,                  # statistics + apply
-                    "svr2_histogram_match_f32": 2}         # iota + rank scatter (the CUB radix-sort passes are library launches)
+                    "svr2_histogram_match_f32": 2,         # iota + rank scatter (the CUB radix-sort passes are library launches)
+                    "svr2_alpha_upscale": 9,               # statistics (3), tap tables (2), resize, Sobel, guided filter (2)
+                    "svr2_sobel_edges_f32": 5}             # statistics (3), Sobel, edge values
 
 
 class Profiler:

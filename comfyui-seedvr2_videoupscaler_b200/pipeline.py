@@ -7,7 +7,9 @@ between phases on the device (no host bounce).  ``upscale_clip`` strings them
 together the way ``generation_phases.py`` does for one clip: 4n+1 temporal pad
 (:109-124), clamp + pad-16 + normalise (``generation_utils.py:72-84``), encode,
 condition = [latent | 1] (``infer.py:54-78``), DiT, decode, crop, optional colour
-correction against the input clip (``generation_phases.py:1249-1319``), [0,1] image format.
+correction against the input clip (``generation_phases.py:1249-1319``), [0,1] image format.  With ``keep_alpha`` an
+RGBA clip keeps its alpha: edge-guided upscaling against the decoded RGB before colour correction (:1142-1217,
+``alpha.py``).
 """
 from __future__ import annotations
 
@@ -15,7 +17,7 @@ from typing import Dict, Optional
 
 import torch
 
-from . import color_fix, preprocess
+from . import alpha, color_fix, preprocess
 from .dit import B200NaDiT, dit_config
 from .vae import B200VideoVAE
 
@@ -114,24 +116,45 @@ class SeedVR2Engine:
     @torch.no_grad()
     def upscale_clip(self, frames: torch.Tensor, noise: Optional[torch.Tensor] = None, seed: int = 42,
                      color_correction: str = "none", resolution: Optional[int] = None,
-                     max_resolution: int = 0) -> torch.Tensor:
+                     max_resolution: int = 0, keep_alpha: bool = False) -> torch.Tensor:
         """frames (T,h,w,3) in [0,1]; ``resolution`` = target shortest edge (None: keep the size, i.e. the frames
         are already at the target resolution).  Returns (T,H,W,3) bf16 in [0,1] on the device.
         ``color_correction``: "none", "lab" (the reference CLI default), "wavelet" or "adain" — matched against the
-        transformed input clip (generation_phases.py:1299-1317)."""
-        sample, style = self.clip_to_sample(frames, noise=noise, seed=seed, resolution=resolution,
-                                            max_resolution=max_resolution)
+        transformed input clip (generation_phases.py:1299-1317).
+        ``keep_alpha``: frames (T,h,w,4) are RGBA; returns (T,H,W,4) with the alpha upscaled against the decoded RGB
+        (generation_phases.py:1142-1217).  Without it a 4th channel is ignored."""
+        rgba = keep_alpha and frames.shape[-1] == 4
+        out = self.clip_to_sample(frames, noise=noise, seed=seed, resolution=resolution, max_resolution=max_resolution,
+                                  keep_alpha=rgba)
+        return self.finish_clip(*out, color_correction=color_correction)
+
+    @staticmethod
+    def finish_clip(sample: torch.Tensor, style: torch.Tensor, src: Optional[torch.Tensor] = None,
+                    color_correction: str = "none") -> torch.Tensor:
+        """Phase 4 for one clip (or slice): optional colour correction, [0,1] image format (T,H,W,3).  ``src``: the
+        input RGBA frames (T,h,w,4) of these output frames; their alpha is upscaled against the decoded sample before
+        the colour correction (which stays RGB-only) and becomes channel 3 of a (T,H,W,4) image."""
+        if src is None:
+            if color_correction != "none":
+                sample = color_fix.apply_color_correction(sample, style, color_correction)
+            return color_fix.sample_to_image(sample)                # t h w c in [0,1]
+        sample = sample.to(torch.bfloat16).contiguous()
+        T, _, H, W = sample.shape
+        image = torch.empty(T, H, W, 4, device=sample.device, dtype=torch.bfloat16)
+        alpha.upscale_into_image(src, sample, image)
         if color_correction != "none":
             sample = color_fix.apply_color_correction(sample, style, color_correction)
-        return color_fix.sample_to_image(sample)                    # t h w c in [0,1]
+        return color_fix.sample_to_image_rgba(sample, image)
 
     @torch.no_grad()
     def clip_to_sample(self, frames: torch.Tensor, noise: Optional[torch.Tensor] = None, seed: int = 42,
-                       resolution: Optional[int] = None, max_resolution: int = 0):
+                       resolution: Optional[int] = None, max_resolution: int = 0, keep_alpha: bool = False):
         """Phases 1-3 for one clip: frames (T,h,w,3) in [0,1] -> (sample, style), both (T,3,H,W) bf16 in [-1,1]:
-        the decoded clip and the transformed input clip it is colour-matched against in phase 4."""
+        the decoded clip and the transformed input clip it is colour-matched against in phase 4.  ``keep_alpha``
+        (frames (T,h,w,4)): (sample, style, src) with src the input frames on the device, unpadded, whose alpha
+        phase 4 upscales."""
         T0 = frames.shape[0]
-        x = frames.to(self.device)
+        x = src = frames.to(self.device)
         x = pad_video_temporal(x)                                   # mirrored tail frames, generation_phases.py:109-124
         # resize (identity when the frames already have the target size) + clamp + pad-16 + normalise + c t h w
         # in one kernel (prepare_video_transforms, generation_utils.py:72-84)
@@ -150,26 +173,32 @@ class SeedVR2Engine:
         del ws, kw
         sample = y[:, :T0, :H0, :W0].permute(1, 0, 2, 3)            # t c h w, the layout of phase 4
         style = x[:, :T0, :H0, :W0].permute(1, 0, 2, 3)            # the transformed input clip in [-1,1]
-        return sample, style
+        return (sample, style, src) if keep_alpha else (sample, style)
 
     @torch.no_grad()
     def upscale_video(self, frames: torch.Tensor, batch_size: int = 5, temporal_overlap: int = 0, seed: int = 42,
                       color_correction: str = "none", resolution: Optional[int] = None,
-                      max_resolution: int = 0) -> torch.Tensor:
+                      max_resolution: int = 0, keep_alpha: bool = False) -> torch.Tensor:
         """A whole video on one GPU the way the reference's four phases do it (generation_phases.py:271-289, 344-358,
         969-1000, 1236-1345): batches of ``batch_size`` frames stepping by ``batch_size - temporal_overlap``, every batch
         seeded identically, the overlap cross-faded into the previous batch's tail, colour correction per batch
-        against its own input frames, [0,1] image format.  Returns (T,H,W,3) bf16."""
+        against its own input frames, [0,1] image format.  Returns (T,H,W,3) bf16.  ``keep_alpha`` with RGBA frames:
+        (T,H,W,4); the alpha of every post-processed slice is upscaled from the input alpha of exactly that slice's
+        frames against its decoded RGB after the cross-fade."""
         from . import shard
+        rgba = keep_alpha and frames.shape[-1] == 4
 
         def clip(a, b):
-            s, st = self.clip_to_sample(frames[a:b], seed=seed, resolution=resolution, max_resolution=max_resolution)
-            return s.contiguous(), st.contiguous()
+            if not rgba:
+                s, st = self.clip_to_sample(frames[a:b], seed=seed, resolution=resolution, max_resolution=max_resolution)
+                return s.contiguous(), st.contiguous()
+            s, st, src = self.clip_to_sample(frames[a:b], seed=seed, resolution=resolution,
+                                             max_resolution=max_resolution, keep_alpha=True)
+            return s.contiguous(), (st.contiguous(), src)
 
         def post(sample, style):
-            if color_correction != "none":
-                sample = color_fix.apply_color_correction(sample, style, color_correction)
-            return color_fix.sample_to_image(sample)
+            style, src = style if rgba else (style, None)
+            return self.finish_clip(sample, style, src, color_correction=color_correction)
 
         return run_batched(frames.shape[0], batch_size, temporal_overlap, clip, shard.blend_overlap, post)
 
@@ -191,9 +220,14 @@ def batch_ranges(total: int, batch_size: int, temporal_overlap: int = 0):
     return out, temporal_overlap
 
 
+def _frames(x, sl: slice):
+    return tuple(t[sl] for t in x) if isinstance(x, tuple) else x[sl]
+
+
 def run_batched(total: int, batch_size: int, temporal_overlap: int, clip_fn, blend_fn, post_fn) -> torch.Tensor:
     """The reference's batch loop with the engine plugged in as callables: ``clip_fn(start, end) -> (sample, style)``
-    ((t,3,H,W) in [-1,1]), ``blend_fn(prev_tail, cur_head)``, ``post_fn(sample, style) -> (t,H,W,3)``.  Decoded batches are
+    ((t,3,H,W) in [-1,1]; ``style`` may be a tuple of per-frame tensors, all sliced along frames alike),
+    ``blend_fn(prev_tail, cur_head)``, ``post_fn(sample, style) -> (t,H,W,C)``.  Decoded batches are
     laid end to end; from the second batch on the first ``overlap`` frames are cross-faded into the tail already written
     and dropped (generation_phases.py:969-1000), and phase 4 then post-processes every batch's slice against its own
     input frames minus those overlap frames (:1249-1263)."""
@@ -213,9 +247,9 @@ def run_batched(total: int, batch_size: int, temporal_overlap: int, clip_fn, ble
                 k -= n
                 if k == 0:
                     break
-            sample, style = sample[overlap:], style[overlap:]
+            sample, style = sample[overlap:], _frames(style, slice(overlap, None))
         samples.append(sample)
-        styles.append(style[: sample.shape[0]])
+        styles.append(_frames(style, slice(None, sample.shape[0])))
         written += sample.shape[0]
     return torch.cat([post_fn(s_, st_) for s_, st_ in zip(samples, styles)], 0)
 
@@ -228,7 +262,8 @@ class GraphedClip:
     train).  All launches go through the C ABI on the current stream with pre-built tensor maps, nothing on the path
     synchronises with the host and the window / RoPE tables are cached per shape, so the whole clip — pre-processing,
     VAE encode, DiT, VAE decode, colour correction, formatting — captures into ONE graph whose intermediates live in
-    the graph's private pool.  ``__call__`` copies the new frames into the static input and replays."""
+    the graph's private pool.  ``__call__`` copies the new frames into the static input and replays.  ``clip_kwargs``
+    are those of ``upscale_clip``; ``keep_alpha=True`` captures the alpha path of RGBA frames as well."""
 
     def __init__(self, engine: "SeedVR2Engine", frames: torch.Tensor, noise: Optional[torch.Tensor] = None,
                  seed: int = 42, warmup: int = 2, **clip_kwargs):

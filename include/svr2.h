@@ -314,6 +314,36 @@ int64_t svr2_resize_scratch_bytes(int h, int w, int H, int W);
 int svr2_resize_bicubic_aa_bf16(const void* in, int in_dtype, int channels_last, int cin, int frames, int h, int w,
                                 void* out, int H, int W, int finish, void* scratch, int64_t scratch_bytes, void* stream);
 
+/* ---- Alpha channel of RGBA clips (edge_guided_alpha_upscale, src/core/alpha_upscaling.py:289-438, called from
+ * generation_phases.py:1142-1217).  All in fp32, no host synchronisation.
+ * Scratch: svr2_alpha_upscale_scratch_bytes(frames, h, w, H, W) bytes.  After a call its first 24 bytes hold
+ *   int32 binary, normalise, normalise_twice, radius; float32 binary_ratio, guide_min
+ * (the branch decisions of :319-334 and of detect_edges_batch :148-149, which the later kernels read on the device). */
+int64_t svr2_alpha_upscale_scratch_bytes(int frames, int h, int w, int H, int W);
+/* Steps of :310-426 for `frames` frames:
+ *   alpha_src [frames,h,w,src_channels] (src_channels 4: RGBA frames, 1: an alpha plane), the alpha is the last
+ *     channel; src_dtype 0 fp32 | 1 bf16 | 2 fp16, rounded to bf16 on load (the clip in the compute dtype, :407-473);
+ *   rgb_up [frames,3,H,W] bf16: the decoded sample before colour correction, the guide (:331-337);
+ *   binary mask = (count(a < 0.1) + count(a > 0.9)) / numel > 0.95 over all frames (:319-324);
+ *   guide = (rgb + 1) / 2 when min(rgb) < 0; Sobel edges of the guide (detect_edges_batch, :125-188, bit-exact);
+ *   base = antialiased bicubic resize of the alpha to H x W, clamp(0, 1) (:342-348);
+ *   guided filter of base by mean(guide) (:191-286), radius 2 (binary) or 3, eps 0.002; binary masks then the
+ *   edge-zone refinement of :370-408; clamp(0, 1).
+ * out_kind 0: out [frames,H,W] fp32;  1: out [frames,H,W,4] bf16, channel 3 written (the RGBA image);
+ *          2: out [frames,H,W] fp32 = the clamped base resize alone (inspection of that step). */
+int svr2_alpha_upscale(const void* alpha_src, int src_dtype, int src_channels, int frames, int h, int w,
+                       const void* rgb_up, int H, int W, void* out, int out_kind, void* scratch, int64_t scratch_bytes,
+                       void* stream);
+/* detect_edges_batch(images, 'sobel') (alpha_upscaling.py:125-188) on rgb_up [frames,3,H,W] bf16 -> edges
+ * [frames,H,W] fp32 in [0,1], bit-exact (OpenCV's integer RGB2GRAY, Sobel with BORDER_REFLECT_101, numpy's fp64
+ * magnitude / per-frame max).  Scratch as for svr2_alpha_upscale. */
+int svr2_sobel_edges_f32(const void* rgb_up, int frames, int H, int W, float* edges, void* scratch,
+                         int64_t scratch_bytes, void* stream);
+/* RGBA formatting (generation_phases.py:1325-1345): sample [frames,3,hw] bf16 -> channels 0..2 of image
+ * [frames,hw,4] bf16 as svr2_sample_to_image_bf16 does; channel 3 (the alpha written by svr2_alpha_upscale with
+ * out_kind 1) is left untouched. */
+int svr2_sample_to_image_rgba_bf16(const void* sample, void* image, int frames, int64_t hw, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
