@@ -6,12 +6,15 @@ meaning and value ranges — for the methods the engine ships:
   ``wavelet_reconstruction(content_feat, style_feat, debug=None)``          (``color_fix.py:187-246``)
   ``adaptive_instance_normalization(content_feat, style_feat)``             (``color_fix.py:94-119``)
   ``lab_color_transfer(content_feat, style_feat, debug, luminance_weight)`` (``color_fix.py:249-365``; CLI default)
+  ``hsv_saturation_histogram_match(content_feat, style_feat, debug=None)``  (``color_fix.py:524-769``)
+  ``wavelet_adaptive_color_correction(content_feat, style_feat, debug=None)`` (``color_fix.py:772-872``)
 
 plus ``sample_to_image`` = ``optimized_sample_to_image_format`` + ``clamp(-1,1)*0.5+0.5``
 (``generation_phases.py:1322-1345``) and ``apply_color_correction`` = the method switch of
 ``generation_phases.py:1299-1317``.  Tensors are ``[T, 3, H, W]`` in ``[-1, 1]`` on the GPU; results are bf16 (the
-pipeline's compute dtype).  Every op is a libsvr2.so kernel (``csrc/post.cu``); there is no torch fallback.
-``hsv`` and ``wavelet_adaptive`` are not part of the engine's path (they raise).
+pipeline's compute dtype).  Every op is a libsvr2.so kernel (``csrc/post.cu``, ``csrc/hsv.cu``); there is no torch
+fallback.  The switch accepts "none", "lab", "wavelet", "adain" and "wavelet_adaptive"; "hsv" still raises there and
+is reached through ``hsv_saturation_histogram_match``.
 """
 from __future__ import annotations
 
@@ -36,29 +39,37 @@ def _check_pair(content: torch.Tensor, style: torch.Tensor):
         raise NotImplementedError(f"content {tuple(content.shape)} and style {tuple(style.shape)} must match")
 
 
-def _wavelet(content: torch.Tensor, style: torch.Tensor) -> torch.Tensor:
+def _wavelet(content: torch.Tensor, style: torch.Tensor, fp32: bool = False) -> torch.Tensor:
+    """bf16 planes in; the reconstruction in bf16 (the reference's compute-dtype pass) or, with ``fp32``, the same
+    pass on fp32 copies of the inputs without intermediate rounding (as wavelet_adaptive runs it), returned fp32."""
     T, _, H, W = content.shape
     planes = T * 3
     st = lib.stream()
-    high = torch.empty_like(content)
-    ping, pong = torch.empty_like(content), torch.empty_like(content)
-    out = torch.empty_like(content)
-    nb = 2.0 * content.numel()
+    dt = torch.float32 if fp32 else torch.bfloat16
+    high = torch.empty_like(content, dtype=dt)
+    ping, pong = torch.empty_like(content, dtype=dt), torch.empty_like(content, dtype=dt)
+    out = torch.empty_like(content, dtype=dt)
+    nb = (4.0 if fp32 else 2.0) * content.numel()
+
+    def level(src, *args, nbytes):
+        if fp32:   # the first level of each pass reads the bf16 clip itself
+            lib.call("svr2_wavelet_level_f32", lib.ptr(src), int(src.dtype == torch.bfloat16), *args, st, nbytes=nbytes)
+        else:
+            lib.call("svr2_wavelet_level_bf16", lib.ptr(src), *args, st, nbytes=nbytes)
+
     # content pass: keep the accumulated high frequencies (color_fix.py:224-225)
     src = content
     for i in range(WAVELET_LEVELS):
         dst = ping if (i % 2 == 0) else pong
-        lib.call("svr2_wavelet_level_bf16", lib.ptr(src), lib.ptr(dst), lib.ptr(high), None, None, planes, H, W,
-                 2 ** i, int(i == 0), st, nbytes=4 * nb)
+        level(src, lib.ptr(dst), lib.ptr(high), None, None, planes, H, W, 2 ** i, int(i == 0), nbytes=4 * nb)
         src = dst
     # style pass: keep the last low-pass (color_fix.py:227-228); its last level also does high + low, clamp (:242-246)
     src = style
     for i in range(WAVELET_LEVELS):
         last = i == WAVELET_LEVELS - 1
         dst = ping if (i % 2 == 0) else pong
-        lib.call("svr2_wavelet_level_bf16", lib.ptr(src), None if last else lib.ptr(dst), None,
-                 lib.ptr(high) if last else None, lib.ptr(out) if last else None, planes, H, W, 2 ** i, 0, st,
-                 nbytes=(3 if last else 2) * nb)
+        level(src, None if last else lib.ptr(dst), None, lib.ptr(high) if last else None,
+              lib.ptr(out) if last else None, planes, H, W, 2 ** i, 0, nbytes=(3 if last else 2) * nb)
         src = dst
     return out
 
@@ -108,6 +119,36 @@ def lab_color_transfer(content_feat: torch.Tensor, style_feat: torch.Tensor, deb
     return out
 
 
+def _hsv_match(c: torch.Tensor, s: torch.Tensor, wavelet=None) -> torch.Tensor:
+    T, _, H, W = c.shape
+    n = T * H * W
+    need = lib.load().svr2_hsv_scratch_bytes(n)
+    if need <= 0:
+        raise lib.Svr2Error(f"HSV colour correction takes fewer than 2^31 pixels per batch, got {n}")
+    scratch = torch.empty(need, device=c.device, dtype=torch.uint8)
+    out = torch.empty_like(c)
+    # bytes per pixel: bins 12 + 44 | sorts of 2 entries (12 B content pairs, 8 B style keys): a histogram read and
+    # 5 read + write passes over 34 key bits, 256 + 176 | match 32 + 8 + 4 | compose 16 (+ 18 for the blend)
+    lib.call("svr2_hsv_saturation_match_bf16", lib.ptr(c), lib.ptr(s), lib.ptr(wavelet), lib.ptr(out), T, H * W,
+             lib.ptr(scratch), need, lib.stream(), nbytes=(566.0 if wavelet is not None else 548.0) * n)
+    return out
+
+
+def hsv_saturation_histogram_match(content_feat: torch.Tensor, style_feat: torch.Tensor, debug=None) -> torch.Tensor:
+    """Hue-conditional saturation histogram matching in HSV (``color_fix.py:524-769``): per 30-degree hue bin with more
+    than 100 pixels on both sides, the content saturations take the style's distribution; hue and value are kept."""
+    _check_pair(content_feat, style_feat)
+    return _hsv_match(_as_planes(content_feat), _as_planes(style_feat))
+
+
+def wavelet_adaptive_color_correction(content_feat: torch.Tensor, style_feat: torch.Tensor, debug=None) -> torch.Tensor:
+    """fp32 wavelet reconstruction with the HSV saturation match blended in where the content is over-saturated
+    against the style and the wavelet result still is (``color_fix.py:772-872``)."""
+    _check_pair(content_feat, style_feat)
+    c, s = _as_planes(content_feat), _as_planes(style_feat)
+    return _hsv_match(c, s, _wavelet(c, s, fp32=True))
+
+
 def sample_to_image(sample: torch.Tensor) -> torch.Tensor:
     """``[T, 3, H, W]`` in [-1, 1] -> ``[T, H, W, 3]`` in [0, 1] (``generation_phases.py:1322-1345``)."""
     x = _as_planes(sample)
@@ -139,6 +180,9 @@ def apply_color_correction(sample: torch.Tensor, input_video: torch.Tensor, colo
         return wavelet_reconstruction(sample, input_video, debug)
     if color_correction == "adain":
         return adaptive_instance_normalization(sample, input_video)
-    if color_correction in ("hsv", "wavelet_adaptive"):
-        raise NotImplementedError(f"color_correction={color_correction!r} is not part of the engine's path")
+    if color_correction == "wavelet_adaptive":
+        return wavelet_adaptive_color_correction(sample, input_video, debug)
+    if color_correction == "hsv":
+        # the kernel ships as hsv_saturation_histogram_match; the switch does not route to it yet
+        raise NotImplementedError("color_correction='hsv': call hsv_saturation_histogram_match directly")
     raise ValueError(f"unknown color_correction {color_correction!r}")

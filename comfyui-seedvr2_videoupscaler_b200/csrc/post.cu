@@ -15,6 +15,9 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
+#include <stdio.h>
+
+#include <type_traits>
 
 #include "svr2_internal.h"
 
@@ -24,25 +27,34 @@ namespace {
 __device__ __forceinline__ float bf2f(__nv_bfloat16 v) { return __bfloat162float(v); }
 __device__ __forceinline__ float rn(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }   // one rounding point
 
+// Storage of the wavelet planes: bf16 rounds at every reference rounding point (the pipeline's compute dtype),
+// fp32 is the same flow without intermediate rounding (wavelet_adaptive_color_correction casts its inputs to
+// fp32 first, color_fix.py:808-812).
+__device__ __forceinline__ float ld(__nv_bfloat16 v) { return bf2f(v); }
+__device__ __forceinline__ float ld(float v) { return v; }
+template <typename T> __device__ __forceinline__ float rnd(float x) { return rn(x); }
+template <> __device__ __forceinline__ float rnd<float>(float x) { return x; }
+template <typename T> __device__ __forceinline__ T cvt(float x) { return __float2bfloat16_rn(x); }
+template <> __device__ __forceinline__ float cvt<float>(float x) { return x; }
+
 // ---------------------------------------------------------------------------------------------------------
-// One wavelet level on `planes` images of H x W (bf16, planar):
-//   low      = rn( sum_{dy,dx} k[dy] k[dx] img[clamp(y + dy r)][clamp(x + dx r)] ),  k = (1,2,1)/4
-//   high     = rn( rn(high + img) - low )          (content pass; `first` => high starts at 0)
-//   out      = clamp( rn(add_to + low), -1, 1 )    (last level of the style pass: content high + style low)
-// The nine products are exact (bf16 x power of two) and the fp32 sum is order-independent up to the last
-// fp32 bit, so `low` matches the reference's conv2d bit for bit in practice.
+// One wavelet level on `planes` images of H x W (planar; img in TIn, the other planes in T):
+//   low      = rnd( sum_{dy,dx} k[dy] k[dx] img[clamp(y + dy r)][clamp(x + dx r)] ),  k = (1,2,1)/4
+//   high     = rnd( rnd(high + img) - low )        (content pass; `first` => high starts at 0)
+//   out      = clamp( rnd(add_to + low), -1, 1 )   (last level of the style pass: content high + style low)
+// bf16: the nine products are exact (bf16 x power of two) and the fp32 sum is order-independent up to the last
+// fp32 bit, so `low` matches the reference's conv2d bit for bit in practice.  fp32: the taps are summed in the
+// order of color_oracle.wavelet_blur (dy outer, dx inner, one rounded add each), so the sum is reproducible.
 // Grid: (ceil(W / 256), H, planes); a thread owns two horizontally adjacent pixels.
-__global__ void __launch_bounds__(128) wavelet_level_kernel(const __nv_bfloat16* __restrict__ img,
-                                                            __nv_bfloat16* __restrict__ low,
-                                                            __nv_bfloat16* __restrict__ high,
-                                                            const __nv_bfloat16* __restrict__ add_to,
-                                                            __nv_bfloat16* __restrict__ out, int H, int W, int r,
-                                                            int first) {
+template <typename TIn, typename T>
+__global__ void __launch_bounds__(128) wavelet_level_kernel(const TIn* __restrict__ img, T* __restrict__ low,
+                                                            T* __restrict__ high, const T* __restrict__ add_to,
+                                                            T* __restrict__ out, int H, int W, int r, int first) {
   const int x0 = (blockIdx.x * 128 + threadIdx.x) * 2;
   if (x0 >= W) return;
   const int y = blockIdx.y;
   const long long plane = (long long)blockIdx.z * H * W;
-  const __nv_bfloat16* p = img + plane;
+  const TIn* p = img + plane;
   const int ym = max(y - r, 0), yp = min(y + r, H - 1);
   const int rows[3] = {ym, y, yp};
   float acc[2] = {0.f, 0.f};
@@ -51,11 +63,22 @@ __global__ void __launch_bounds__(128) wavelet_level_kernel(const __nv_bfloat16*
     const int x = min(x0 + px, W - 1);
     const int xm = max(x - r, 0), xp = min(x + r, W - 1);
     float s = 0.f;
+    if constexpr (std::is_same<T, float>::value) {
+      const int cols[3] = {xm, x, xp};
+      const float k[3] = {0.25f, 0.5f, 0.25f};
 #pragma unroll
-    for (int i = 0; i < 3; ++i) {
-      const __nv_bfloat16* row = p + (long long)rows[i] * W;
-      const float h = 0.25f * bf2f(row[xm]) + 0.5f * bf2f(row[x]) + 0.25f * bf2f(row[xp]);
-      s += (i == 1 ? 0.5f : 0.25f) * h;
+      for (int i = 0; i < 3; ++i) {
+        const TIn* row = p + (long long)rows[i] * W;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) s = __fadd_rn(s, __fmul_rn(ld(row[cols[j]]), k[i] * k[j]));
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        const TIn* row = p + (long long)rows[i] * W;
+        const float h = 0.25f * ld(row[xm]) + 0.5f * ld(row[x]) + 0.25f * ld(row[xp]);
+        s += (i == 1 ? 0.5f : 0.25f) * h;
+      }
     }
     acc[px] = s;
   }
@@ -64,17 +87,17 @@ __global__ void __launch_bounds__(128) wavelet_level_kernel(const __nv_bfloat16*
 #pragma unroll
   for (int px = 0; px < 2; ++px) {
     if (px == 1 && !two) break;
-    const float lo = rn(acc[px]);
+    const float lo = rnd<T>(acc[px]);
     if (add_to) {
-      const float v = rn(bf2f(add_to[o + px]) + lo);
-      out[o + px] = __float2bfloat16_rn(fminf(fmaxf(v, -1.f), 1.f));
+      const float v = rnd<T>(ld(add_to[o + px]) + lo);
+      out[o + px] = cvt<T>(fminf(fmaxf(v, -1.f), 1.f));
     } else {
-      low[o + px] = __float2bfloat16_rn(lo);
+      low[o + px] = cvt<T>(lo);
     }
     if (high) {
-      const float im = bf2f(p[(long long)y * W + x0 + px]);
-      const float hprev = first ? 0.f : bf2f(high[o + px]);
-      high[o + px] = __float2bfloat16_rn(rn(hprev + im) - lo);
+      const float im = ld(p[(long long)y * W + x0 + px]);
+      const float hprev = first ? 0.f : ld(high[o + px]);
+      high[o + px] = cvt<T>(rnd<T>(hprev + im) - lo);
     }
   }
 }
@@ -302,20 +325,48 @@ inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 using namespace svr2;
 
-extern "C" int svr2_wavelet_level_bf16(const void* img, void* low, void* high, const void* add_to, void* out,
-                                       int planes, int H, int W, int radius, int first, void* stream) {
-  if (planes <= 0 || H <= 0 || W <= 0) return set_error(SVR2_ERR_ARG, "svr2_wavelet_level_bf16: empty image");
-  if (planes > 65535 || H > 65535) return set_error(SVR2_ERR_ARG, "svr2_wavelet_level_bf16: planes, H <= 65535");
-  if ((add_to != nullptr) != (out != nullptr)) return set_error(SVR2_ERR_ARG, "add_to and out go together");
-  if (!add_to && !low) return set_error(SVR2_ERR_ARG, "svr2_wavelet_level_bf16: low is required");
+// argument checks shared by both storage types; returns the capped dilation, or -1 after set_error
+static int wavelet_level_radius(const char* fn, const void* low, const void* add_to, const void* out, int planes,
+                                int H, int W, int radius) {
+  const char* why = nullptr;
+  if (planes <= 0 || H <= 0 || W <= 0) why = "empty image";
+  else if (planes > 65535 || H > 65535) why = "planes, H <= 65535";
+  else if ((add_to != nullptr) != (out != nullptr)) why = "add_to and out go together";
+  else if (!add_to && !low) why = "low is required";
+  if (why) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "%s: %s", fn, why);
+    set_error(SVR2_ERR_ARG, buf);
+    return -1;
+  }
   int cap = (H < W ? H : W) / 8;                          // max_safe_radius, color_fix.py:136-140
   if (cap < 1) cap = 1;
-  const int r = radius > cap ? cap : radius;
+  return radius > cap ? cap : radius;
+}
+
+extern "C" int svr2_wavelet_level_bf16(const void* img, void* low, void* high, const void* add_to, void* out,
+                                       int planes, int H, int W, int radius, int first, void* stream) {
+  const int r = wavelet_level_radius("svr2_wavelet_level_bf16", low, add_to, out, planes, H, W, radius);
+  if (r < 0) return SVR2_ERR_ARG;
   dim3 grid((W + 255) / 256, H, planes);
   wavelet_level_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)img, (__nv_bfloat16*)low,
                                                                (__nv_bfloat16*)high, (const __nv_bfloat16*)add_to,
                                                                (__nv_bfloat16*)out, H, W, r, first);
   return check_launch("wavelet_level");
+}
+
+extern "C" int svr2_wavelet_level_f32(const void* img, int img_bf16, float* low, float* high, const float* add_to,
+                                      float* out, int planes, int H, int W, int radius, int first, void* stream) {
+  const int r = wavelet_level_radius("svr2_wavelet_level_f32", low, add_to, out, planes, H, W, radius);
+  if (r < 0) return SVR2_ERR_ARG;
+  dim3 grid((W + 255) / 256, H, planes);
+  if (img_bf16)
+    wavelet_level_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)img, low, high, add_to, out, H,
+                                                                 W, r, first);
+  else
+    wavelet_level_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>((const float*)img, low, high, add_to, out, H, W, r,
+                                                                 first);
+  return check_launch("wavelet_level_f32");
 }
 
 extern "C" int svr2_adain_bf16(const void* content, const void* style, void* out, int planes, int64_t hw,

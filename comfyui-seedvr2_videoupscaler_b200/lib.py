@@ -80,6 +80,9 @@ SIGNATURES = {
     "svr2_conv_tap_gather": [_P, c_int64, c_int, _P, c_int, c_int, c_int, _P, c_int, _P],
     "svr2_im2col3_bf16": [_P, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P],
     "svr2_wavelet_level_bf16": [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P],
+    "svr2_wavelet_level_f32": [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P],
+    "svr2_hsv_scratch_bytes": [c_int64],
+    "svr2_hsv_saturation_match_bf16": [_P, _P, _P, _P, c_int, c_int64, _P, c_int64, _P],
     "svr2_adain_bf16": [_P, _P, _P, c_int, c_int64, _P, _P],
     "svr2_rgb_to_lab_f32": [_P, _P, c_int, c_int64, _P],
     "svr2_lab_to_rgb_bf16": [_P, _P, _P, _P, c_float, _P, c_int, c_int64, _P],
@@ -143,6 +146,7 @@ KERNELS_PER_CALL = {"svr2_groupnorm_bf16": 3, "svr2_groupnorm_from_stats_bf16": 
                     "svr2_resize_bicubic_aa_bf16": 3,      # two tap-table kernels + the resize
                     "svr2_adain_bf16": 2,                  # statistics + apply
                     "svr2_histogram_match_f32": 2,         # iota + rank scatter (the CUB radix-sort passes are library launches)
+                    "svr2_hsv_saturation_match_bf16": 3,   # bins, match, compose (plus a memset and the CUB sorts)
                     "svr2_alpha_upscale": 9,               # statistics (3), tap tables (2), resize, Sobel, guided filter (2)
                     "svr2_sobel_edges_f32": 5}             # statistics (3), Sobel, edge values
 

@@ -119,8 +119,8 @@ class SeedVR2Engine:
                      max_resolution: int = 0, keep_alpha: bool = False) -> torch.Tensor:
         """frames (T,h,w,3) in [0,1]; ``resolution`` = target shortest edge (None: keep the size, i.e. the frames
         are already at the target resolution).  Returns (T,H,W,3) bf16 in [0,1] on the device.
-        ``color_correction``: "none", "lab" (the reference CLI default), "wavelet" or "adain" — matched against the
-        transformed input clip (generation_phases.py:1299-1317).
+        ``color_correction``: "none", "lab" (the reference CLI default), "wavelet", "adain" or "wavelet_adaptive" —
+        matched against the transformed input clip (generation_phases.py:1299-1317).
         ``keep_alpha``: frames (T,h,w,4) are RGBA; returns (T,H,W,4) with the alpha upscaled against the decoded RGB
         (generation_phases.py:1142-1217).  Without it a 4th channel is ignored."""
         rgba = keep_alpha and frames.shape[-1] == 4

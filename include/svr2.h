@@ -264,6 +264,11 @@ int svr2_im2col3_bf16(const void* x, int T, int H, int W, int C, int ld_in, void
  *   of wavelet_reconstruction (color_fix.py:187-246) fused into the last level of the style pass. */
 int svr2_wavelet_level_bf16(const void* img, void* low, void* high, const void* add_to, void* out, int planes, int H,
                             int W, int radius, int first, void* stream);
+/* The same level in fp32, as wavelet_reconstruction runs on the fp32 copies of wavelet_adaptive_color_correction
+ * (color_fix.py:808-812): no intermediate rounding, the nine taps summed dy-major in fp32.  img is bf16 when
+ * img_bf16 != 0 (the first level reads the clip itself), else fp32; low / high / add_to / out are fp32. */
+int svr2_wavelet_level_f32(const void* img, int img_bf16, float* low, float* high, const float* add_to, float* out,
+                           int planes, int H, int W, int radius, int first, void* stream);
 /* adaptive_instance_normalization (color_fix.py:72-119): per plane, out = (c - mean_c) / std_c * std_s + mean_s with
  * unbiased variance, eps 1e-5 and the reference's bf16 rounding points.  stats_scratch: planes * 4 floats. */
 int svr2_adain_bf16(const void* content, const void* style, void* out, int planes, int64_t hw, float* stats_scratch,
@@ -279,6 +284,21 @@ int svr2_lab_to_rgb_bf16(const float* L_content, const float* L_matched, const f
 int64_t svr2_histogram_match_scratch_bytes(int64_t n);
 int svr2_histogram_match_f32(const float* source, const float* reference, float* out, int64_t n, void* scratch,
                              int64_t scratch_bytes, void* stream);
+/* hsv_saturation_histogram_match (color_fix.py:524-611, 614-769) for equal shapes: content / style [frames,3,hw] bf16
+ * in [-1,1], n = frames * hw < 2^31 pixels, the histograms taken over all frames together.  RGB -> HSV in fp32; per
+ * hue bin of 1/12 (bin 0 also takes h >= 11/12, and bin 11's match wins for those pixels) with more than 100 content
+ * and 100 style pixels, the content saturation of rank r gets the style saturation of rank r (equal counts) or of
+ * rank (linspace(0, 1, n_content)[r] * (n_style - 1)).long() in fp32 (torch's CUDA linspace); saturation ties are
+ * broken by pixel index.  HSV -> RGB, clamp, [-1,1] -> out bf16.
+ * wavelet != NULL (fp32 [frames,3,hw], svr2_wavelet_level_f32's reconstruction): wavelet_adaptive_color_correction
+ * (color_fix.py:772-872) instead: out = bf16(wav * (1 - w) + hsv * w), w = clamp(sigmoid(5 * ((sat(content) -
+ * sat(style)) - 0.15)) * ((sat(wav) - sat(style)) > 0.075), 0, 1), the fp32 hsv result kept on chip.
+ * Scratch: svr2_hsv_scratch_bytes(n) bytes (0 for n outside [1, 2^31)); its first 256 bytes are a header written by
+ * the call: u32 content_count[12], u32 style_count[12] (bin sizes; a wrap-around pixel counts in bins 0 and 11),
+ * u32 qualify[12]. */
+int64_t svr2_hsv_scratch_bytes(int64_t n);
+int svr2_hsv_saturation_match_bf16(const void* content, const void* style, const float* wavelet, void* out, int frames,
+                                   int64_t hw, void* scratch, int64_t scratch_bytes, void* stream);
 /* final formatting (generation_phases.py:1322-1345): sample [frames,3,hw] bf16 -> image [frames,hw,3] bf16,
  * clamp(-1,1) * 0.5 + 0.5 */
 int svr2_sample_to_image_bf16(const void* sample, void* image, int frames, int64_t hw, void* stream);
