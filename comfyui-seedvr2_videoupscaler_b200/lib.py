@@ -100,6 +100,8 @@ SIGNATURES = {
     "svr2_alpha_upscale": [_P, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int64, _P],
     "svr2_sobel_edges_f32": [_P, c_int, c_int, c_int, _P, _P, c_int64, _P],
     "svr2_sample_to_image_rgba_bf16": [_P, _P, c_int, c_int64, _P],
+    "svr2_input_noise_bf16": [_P, _P, c_int, _P, c_int, c_int64, c_float, c_float, _P],
+    "svr2_sr_condition_bf16": [_P, _P, _P, _P, _P, _P, c_int64, c_int, _P],
 }
 
 _lib = None
@@ -148,7 +150,9 @@ KERNELS_PER_CALL = {"svr2_groupnorm_bf16": 3, "svr2_groupnorm_from_stats_bf16": 
                     "svr2_histogram_match_f32": 2,         # iota + rank scatter (the CUB radix-sort passes are library launches)
                     "svr2_hsv_saturation_match_bf16": 3,   # bins, match, compose (plus a memset and the CUB sorts)
                     "svr2_alpha_upscale": 9,               # statistics (3), tap tables (2), resize, Sobel, guided filter (2)
-                    "svr2_sobel_edges_f32": 5}             # statistics (3), Sobel, edge values
+                    "svr2_sobel_edges_f32": 5,             # statistics (3), Sobel, edge values
+                    "svr2_input_noise_bf16": 1,            # one blend pass
+                    "svr2_sr_condition_bf16": 1}           # one pass writes the DiT input rows
 
 
 class Profiler:

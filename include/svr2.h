@@ -364,6 +364,26 @@ int svr2_sobel_edges_f32(const void* rgb_up, int frames, int H, int W, float* ed
  * out_kind 1) is left untouched. */
 int svr2_sample_to_image_rgba_bf16(const void* sample, void* image, int frames, int64_t hw, void* stream);
 
+/* ---- Generation noise (generation_phases.py:415-431, 679-704).  Each reference op rounds before the next reads it
+ * (no FMA contraction); no host synchronisation.
+ * Input noise (:416-429), out of place: x, out [3,frames,plane] bf16 (the transformed clip, plane = Hp*Wp < 2^31);
+ * noise: the raw standard-normal draw, in the memory order of the reference's randn_like on its transformed clip:
+ *   noise_layout 0: [frames,3,plane]  a batch the reference padded to 4n+1 frames and then resized or padded to 16
+ *                1: [3,frames,plane]  a batch padded to 4n+1 frames that was neither resized nor spatially padded
+ *                2: [frames,plane,3]  a batch of 4n+1 frames as it came (the frames' t h w c memory is kept);
+ * out = bf16(bf16(x*c1) + bf16(bf16(x + bf16(noise*0.05f))*c2)), c1 = (float)(1 - b), c2 = (float)b,
+ * b = input_noise_scale * 0.5. */
+int svr2_input_noise_bf16(const void* x, const void* noise, int noise_layout, void* out, int frames, int64_t plane,
+                          float c1, float c2, void* stream);
+/* DiT input of task "sr" (get_condition, infer.py:54-78): out [rows, 2*channels+1] bf16 = [noise | cond | 1] per row;
+ * noise, latent [rows,channels] bf16 (rows = T'*h*w, channels <= 64, rows*(2*channels+1) < 2^31).
+ * latent_noise NULL: cond = latent.  Otherwise latent_noise [channels,rows] bf16 (channel-major: the second draw r of
+ * :683 in the reference's memory order), coef_a / coef_b one fp32 each on the device (the lerp schedule's A(t), B(t)
+ * at the shifted timestep of :688-693): aug = bf16(bf16(noise*0.1f) + bf16(r*0.05f)),
+ * cond = bf16(fadd(fmul(A, latent), fmul(B, aug))). */
+int svr2_sr_condition_bf16(const void* noise, const void* latent, const void* latent_noise, const float* coef_a,
+                           const float* coef_b, void* out, int64_t rows, int channels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
