@@ -23,7 +23,7 @@ from typing import Dict, List, Tuple
 
 import torch
 
-from . import lib
+from . import lib, weights
 from .attention import FlashAttentionVarlen
 from .lib import EPI_GELU, EPI_SILU, EPI_SWIGLU
 from .module import EngineModule
@@ -247,6 +247,7 @@ class B200NaDiT(EngineModule):
         return sd[key].to(self.device, torch.float32).contiguous()
 
     def _load(self, sd):
+        sd = weights.dequantizing(sd, self.device)   # GGUF entries: dense fp16 on the device, one key at a time
         cfg, dev = self.cfg, self.device
         d = cfg["dim"]
         W: Dict[str, torch.Tensor] = {}

@@ -102,6 +102,8 @@ SIGNATURES = {
     "svr2_sample_to_image_rgba_bf16": [_P, _P, c_int, c_int64, _P],
     "svr2_input_noise_bf16": [_P, _P, c_int, _P, c_int, c_int64, c_float, c_float, _P],
     "svr2_sr_condition_bf16": [_P, _P, _P, _P, _P, _P, c_int64, c_int, _P],
+    "svr2_gguf_type_size": [c_int, POINTER(c_int), POINTER(c_int)],
+    "svr2_gguf_dequant_f16": [c_int, _P, c_int64, _P, _P],
 }
 
 _lib = None

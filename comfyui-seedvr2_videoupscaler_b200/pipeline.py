@@ -427,11 +427,15 @@ def build_synthetic_engine(variant="3b", device="cuda", seed=1234, txt_len=58) -
 
 
 def build_engine(dit_checkpoint: str, vae_checkpoint: str, txt_embed, device="cuda") -> SeedVR2Engine:
-    """Engine from checkpoint files: DiT ``seedvr2_ema_{3b,7b}_{fp16,fp8_e4m3fn}.safetensors``, VAE
+    """Engine from checkpoint files: DiT ``seedvr2_ema_{3b,7b}_{fp16,fp8_e4m3fn}.safetensors`` or a GGUF file
+    (``seedvr2_ema_{3b,7b}-Q4_K_M.gguf`` …, dequantised on the device while the engine loads it), VAE
     ``ema_vae_fp16.safetensors`` (``model_registry.py:40-75``) and the positive text embedding (``pos_emb.pt``,
     ``generation_utils.py:load_text_embeddings``) given as a path or tensor."""
     from . import weights
-    dit_sd = weights.load_state_dict(dit_checkpoint)
+    if dit_checkpoint.lower().endswith(".gguf"):
+        dit_sd = weights.load_gguf(dit_checkpoint)
+    else:
+        dit_sd = weights.load_state_dict(dit_checkpoint)
     cfg = dit_config(weights.detect_dit_variant(dit_sd))
     vae_sd = weights.load_state_dict(vae_checkpoint)
     txt = torch.load(txt_embed, map_location="cpu", weights_only=True) if isinstance(txt_embed, str) else txt_embed

@@ -384,6 +384,15 @@ int svr2_input_noise_bf16(const void* x, const void* noise, int noise_layout, vo
 int svr2_sr_condition_bf16(const void* noise, const void* latent, const void* latent_noise, const float* coef_a,
                            const float* coef_b, void* out, int64_t rows, int channels, void* stream);
 
+/* ---- GGUF block dequantization (gguf_dequant.py:146-342), done once when a GGUF DiT checkpoint is loaded.
+ * Types by GGML id: Q4_0 2, Q4_1 3, Q5_0 6, Q5_1 7, Q8_0 8, Q2_K 10, Q3_K 11, Q4_K 12, Q5_K 13, Q6_K 14, BF16 30.
+ * GGML block sizes (elements and bytes per block); SVR2_ERR_ARG for a type the engine does not dequantize. */
+int svr2_gguf_type_size(int ggml_type, int* block_elems, int* block_bytes);
+/* blocks: n_elements / block_elems consecutive blocks (device, 4-byte aligned); out: n_elements fp16 (16-byte aligned).
+ * Bit-exact with the reference's float16 block functions: each product / sum / difference computed in fp32 and rounded
+ * to fp16 before the next reads it (no FMA); BF16 is widened to fp32 and rounded to fp16 (out of range: +-inf). */
+int svr2_gguf_dequant_f16(int ggml_type, const void* blocks, int64_t n_elements, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
