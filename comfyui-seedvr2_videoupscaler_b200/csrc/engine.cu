@@ -292,11 +292,85 @@ Geometry* geometry(svr2_engine* e, int T, int Hp, int Wp, int l) {
   return g;
 }
 
+// bytes a tensor of the handle occupies: dense, or whole blocks of a compressed format
+size_t tensor_bytes(const Tensor& t) {
+  int be = 0, bb = 0;
+  if (t.dtype >= 3 && weight_format_size(t.dtype, &be, &bb)) return (size_t)(t.numel() / be) * bb;
+  return (size_t)t.numel() * dtype_size(t.dtype);
+}
+
+// The staging slot (svr2.h, "compressed matrices"): which matrices of every block are expanded before the block runs,
+// where they land in the slot, and the slot's size.  A matrix whose sources are those of an earlier matrix of the same
+// block (the 3B layers whose video and text streams share weights) shares its bytes.
+bool build_slot_plan(svr2_engine* e, char* err, size_t err_len) {
+  e->slot_plan.clear();
+  e->slot_bytes = 0;
+  if (e->desc.variant == 2) return true;
+  e->slot_plan.resize(e->desc.layers > 0 ? e->desc.layers : 0);
+  for (int i = 0; i < e->desc.layers; ++i) {
+    std::vector<SlotMatrix>& slots = e->slot_plan[i];
+    size_t off = 0;
+    for (const char* s : {"vid", "txt"})
+      for (const char* n : {"qkv.w", "out.w", "mlp_in.w", "mlp_out.w"}) {
+        SlotMatrix m;
+        m.name = std::to_string(i) + "." + s + "." + n;
+        const Tensor* whole = find(e, m.name);
+        const Tensor *gate = nullptr, *in = nullptr;
+        if (whole && whole->dtype >= 3) {
+          if (whole->rank != 2) {
+            snprintf(err, err_len, "svr2_load_weights: compressed matrix '%s' must have rank 2", m.name.c_str());
+            return false;
+          }
+          m.cols = whole->shape[1];
+          m.parts.push_back({whole->ptr, whole->dtype, whole->shape[0], whole->shape[0], whole->shape[0], 0});
+        } else if (!whole && (gate = find(e, m.name + ".gate")) && (in = find(e, m.name + ".in"))) {
+          if (gate->dtype < 2 || in->dtype < 2 || gate->rank != 2 || in->rank != 2 || gate->shape[0] != in->shape[0] ||
+              gate->shape[1] != in->shape[1] || gate->shape[0] % 128) {
+            snprintf(err, err_len, "svr2_load_weights: '%s.gate' / '.in' must be fp16, fp8_e4m3fn or GGML matrices of one "
+                     "shape with a multiple of 128 rows", m.name.c_str());
+            return false;
+          }
+          m.cols = gate->shape[1];
+          m.parts.push_back({gate->ptr, gate->dtype, gate->shape[0], 128, 256, 0});
+          m.parts.push_back({in->ptr, in->dtype, in->shape[0], 128, 256, 128});
+        } else {
+          continue;
+        }
+        int64_t rows = 0;
+        for (const SlotPart& p : m.parts) {
+          int be = 0, bb = 0;
+          weight_format_size(p.format, &be, &bb);
+          if (p.rows <= 0 || m.cols <= 0 || m.cols % (be > 8 ? be : 8)) {
+            snprintf(err, err_len, "svr2_load_weights: compressed matrix '%s' must have a row length that is a multiple "
+                     "of its block size and of 8", m.name.c_str());
+            return false;
+          }
+          rows += p.rows;
+        }
+        for (const SlotMatrix& prev : slots)
+          if (prev.parts.size() == m.parts.size() && prev.parts[0].src == m.parts[0].src &&
+              prev.parts.back().src == m.parts.back().src) {
+            m.off = prev.off;
+            m.parts.clear();
+            break;
+          }
+        if (!m.parts.empty()) {
+          m.off = off;
+          off += align_up((size_t)rows * m.cols * 2);
+        }
+        slots.push_back(m);
+      }
+    e->slot_bytes = e->slot_bytes > off ? e->slot_bytes : off;
+  }
+  return true;
+}
+
 // workspace plan of one forward (bump allocation, bytes)
 struct Plan {
-  size_t xp, x, t, a_v, a_t, qkv_t, qkv_v, q, k, v, o_all, o_t, h_v, h_t, mm, z, zt, v64, total;
+  size_t xp, x, t, a_v, a_t, qkv_t, qkv_v, q, k, v, o_all, o_t, h_v, h_t, mm, z, zt, v64, slot, total;
 };
-Plan make_plan(const svr2_model_desc& d, int T, int H, int W, int l, int max_total, int max_rows, bool fuse_qkv) {
+Plan make_plan(const svr2_model_desc& d, int T, int H, int W, int l, int max_total, int max_rows, bool fuse_qkv,
+               size_t slot_bytes) {
   const size_t L = (size_t)T * (H / 2) * (W / 2), dim = d.dim, inner = (size_t)d.heads * 128;
   const size_t hid = d.mlp_kind == 0 ? (size_t)d.mlp_hidden : (size_t)d.mlp_hidden;
   Plan p{};
@@ -320,6 +394,7 @@ Plan make_plan(const svr2_model_desc& d, int T, int H, int W, int l, int max_tot
   p.z = take(L * hid * 2);
   p.zt = take((size_t)l * hid * 2);
   p.v64 = take(L * (size_t)d.out_ch * 4 * 2);
+  p.slot = take(slot_bytes);       // 0 bytes when every matrix is resident bf16: the plan is the same as without it
   p.total = off;
   return p;
 }
@@ -380,7 +455,9 @@ extern "C" int svr2_load_weights(svr2_t* e, const svr2_tensor_desc* tensors, siz
   int rc = SVR2_OK;
   for (size_t i = 0; i < n && rc == SVR2_OK; ++i) {
     const svr2_tensor_desc& d = tensors[i];
-    if (!d.name || !d.data || d.rank < 1 || d.rank > 5 || d.dtype < 0 || d.dtype > 2) {
+    int be = 0, bb = 0;
+    if (!d.name || !d.data || d.rank < 1 || d.rank > 5 || d.dtype < 0 ||
+        (d.dtype > 2 && !weight_format_size(d.dtype, &be, &bb))) {
       rc = fail(e, SVR2_ERR_ARG, "svr2_load_weights: bad tensor descriptor");
       break;
     }
@@ -391,7 +468,7 @@ extern "C" int svr2_load_weights(svr2_t* e, const svr2_tensor_desc* tensors, siz
     auto old = e->w.find(d.name);
     if (old != e->w.end() && old->second.owned) cudaFree(old->second.ptr);
     if (copy) {
-      const size_t bytes = (size_t)t.numel() * dtype_size(t.dtype);
+      const size_t bytes = tensor_bytes(t);
       if (cudaMalloc(&t.ptr, bytes ? bytes : 1) != cudaSuccess ||
           cudaMemcpy(t.ptr, d.data, bytes, cudaMemcpyDefault) != cudaSuccess) {
         rc = fail(e, SVR2_ERR_CUDA, "svr2_load_weights: allocation / copy failed");
@@ -409,6 +486,8 @@ extern "C" int svr2_load_weights(svr2_t* e, const svr2_tensor_desc* tensors, siz
     delete kv.second;
   }
   e->geo.clear();
+  char msg[256];
+  if (rc == SVR2_OK && !build_slot_plan(e, msg, sizeof msg)) rc = fail(e, SVR2_ERR_ARG, msg);
   cudaSetDevice(cur);
   return rc;
 }
@@ -426,7 +505,7 @@ extern "C" size_t svr2_workspace_bytes(svr2_t* e, int T, int H, int W, int txt_l
   }
   const size_t max_rows = (size_t)T * Hp * Wp + max_win * txt_len;
   const int nfreq = e->desc.variant == 1 ? 10 : 21;
-  return make_plan(e->desc, T, H, W, txt_len, (int)max_total, (int)max_rows, fuse_qkv_ok(e, nfreq)).total;
+  return make_plan(e->desc, T, H, W, txt_len, (int)max_total, (int)max_rows, fuse_qkv_ok(e, nfreq), e->slot_bytes).total;
 }
 
 // One NaDiT forward: vid [T*H*W, in_ch] bf16 (latent pixels, channels last), txt [txt_len, txt_in_dim] bf16 ->
@@ -466,7 +545,7 @@ static int dit_forward_impl(svr2_t* e, const void* vid, const void* txt, int T, 
   const bool fuse = fuse_qkv_ok(e, g->nfreq);
   const int max_total = g->lay[0].total > g->lay[1].total ? g->lay[0].total : g->lay[1].total;
   const int max_win = g->lay[0].n_win > g->lay[1].n_win ? g->lay[0].n_win : g->lay[1].n_win;
-  const Plan P = make_plan(D, T, H, W, l, max_total, L + max_win * l, fuse);
+  const Plan P = make_plan(D, T, H, W, l, max_total, L + max_win * l, fuse, e->slot_bytes);
   if (ext_ws) {
     if (ext_ws_bytes < P.total) return fail(e, SVR2_ERR_ARG, "svr2_dit_forward_ws: workspace smaller than svr2_workspace_bytes()");
   } else if (P.total > e->workspace_bytes) {
@@ -505,13 +584,28 @@ static int dit_forward_impl(svr2_t* e, const void* vid, const void* txt, int T, 
     const Layout& lay = g->lay[i & 1];
     const RopeTable& tab = g->tables[g->table_of_layer[i]];
     auto Wl = [&](const char* s, const char* n) { return Wt("%d.%s.%s", i, s, n); };
+    // compressed matrices of this block: expanded to bf16 into the slot now (stream order puts this after the previous
+    // block's GEMMs, which read the same slot); Wm finds a block matrix there, or resident among the weights
+    static const std::vector<SlotMatrix> none;
+    const std::vector<SlotMatrix>& slots = (size_t)i < e->slot_plan.size() ? e->slot_plan[i] : none;
+    char* slot = ws + P.slot;
+    for (const SlotMatrix& m : slots)
+      for (const SlotPart& p : m.parts)
+        CK(svr2_weight_expand_bf16(p.format, p.src, p.rows, m.cols, slot + m.off, p.group, p.stride, p.offset, stream));
+    auto Wm = [&](const char* s, const char* n) -> const void* {
+      snprintf(name, sizeof name, "%d.%s.%s", i, s, n);
+      for (const SlotMatrix& m : slots)
+        if (m.name == name) return slot + m.off;
+      const Tensor* t = find(e, name);
+      return t ? t->ptr : nullptr;
+    };
     // ---- attention branch (mmsr_block.py:107-114)
     const void *sc_v = Wl("vid", "attn_scale"), *sh_v = Wl("vid", "attn_shift");
     const void *sc_t = Wl("txt", "attn_scale"), *sh_t = Wl("txt", "attn_shift");
     NEED(sc_v, "<i>.vid.attn_scale"); NEED(sh_v, "<i>.vid.attn_shift"); NEED(sc_t, "<i>.txt.attn_scale"); NEED(sh_t, "<i>.txt.attn_shift");
     CK(svr2_rmsnorm_ada_bf16(x, B(P.a_v), L, d, D.eps, nullptr, (const float*)sc_v, (const float*)sh_v, 0, stream));
     CK(svr2_rmsnorm_ada_bf16(t, B(P.a_t), l, d, D.eps, nullptr, (const float*)sc_t, (const float*)sh_t, 0, stream));
-    const void *wqkv_v = Wl("vid", "qkv.w"), *wqkv_t = Wl("txt", "qkv.w");
+    const void *wqkv_v = Wm("vid", "qkv.w"), *wqkv_t = Wm("txt", "qkv.w");
     const void *nq_v = Wl("vid", "nq"), *nk_v = Wl("vid", "nk"), *nq_t = Wl("txt", "nq"), *nk_t = Wl("txt", "nk");
     const void* nqk_v = Wl("vid", "nqk");
     NEED(wqkv_v, "<i>.vid.qkv.w"); NEED(wqkv_t, "<i>.txt.qkv.w"); NEED(nq_v, "<i>.vid.nq"); NEED(nk_v, "<i>.vid.nk");
@@ -533,7 +627,7 @@ static int dit_forward_impl(svr2_t* e, const void* vid, const void* txt, int T, 
                              lay.out_row_map, stream));
     char* o_txt = reinterpret_cast<char*>(B(P.o_all)) + (size_t)L * inner * 2;
     CK(svr2_txt_window_mean_bf16(o_txt, B(P.o_t), lay.n_win, l, inner, stream));
-    const void *wo_v = Wl("vid", "out.w"), *bo_v = Wl("vid", "out.b"), *wo_t = Wl("txt", "out.w"), *bo_t = Wl("txt", "out.b");
+    const void *wo_v = Wm("vid", "out.w"), *bo_v = Wl("vid", "out.b"), *wo_t = Wm("txt", "out.w"), *bo_t = Wl("txt", "out.b");
     const void *ga_v = Wl("vid", "attn_gate"), *ga_t = last ? nullptr : Wl("txt", "attn_gate");
     NEED(wo_v, "<i>.vid.out.w"); NEED(bo_v, "<i>.vid.out.b"); NEED(wo_t, "<i>.txt.out.w"); NEED(bo_t, "<i>.txt.out.b"); NEED(ga_v, "<i>.vid.attn_gate");
     if (!last) NEED(ga_t, "<i>.txt.attn_gate");
@@ -542,7 +636,7 @@ static int dit_forward_impl(svr2_t* e, const void* vid, const void* txt, int T, 
     // ---- MLP branch (mmsr_block.py:116-126); the outputs land in the buffers that held this layer's inputs
     auto mlp = [&](const char* s, void* hh, void* yy, int rows, void* zbuf) -> int {
       const void *msc = Wl(s, "mlp_scale"), *msh = Wl(s, "mlp_shift"), *mg = Wl(s, "mlp_gate");
-      const void *w1 = Wl(s, "mlp_in.w"), *w2 = Wl(s, "mlp_out.w");
+      const void *w1 = Wm(s, "mlp_in.w"), *w2 = Wm(s, "mlp_out.w");
       if (!msc || !msh || !mg || !w1 || !w2) { snprintf(e->err, sizeof e->err, "svr2_dit_forward: MLP weights of layer %d (%s) not loaded", i, s); return set_error(SVR2_ERR_ARG, e->err); }
       int r = svr2_rmsnorm_ada_bf16(hh, B(P.mm), rows, d, D.eps, nullptr, (const float*)msc, (const float*)msh, 1, stream);
       if (r) return r;

@@ -1,5 +1,7 @@
 // GGUF block dequantization to fp16 (gguf_dequant.py:146-342): the eleven block formats the reference's
-// `dequantize_functions` table handles, decoded once at load so the DiT loader receives dense fp16 tensors.
+// `dequantize_functions` table handles, decoded once at load so the DiT loader receives dense fp16 tensors; and, at the
+// end of the file, the expansion of GGUF / fp8 / fp16 weight matrices straight to bf16 in the engine layout, which runs
+// per transformer block when the weights stay compressed in device memory.
 //
 // Rounding: the reference runs every block function with dtype float16, so each torch op is one Half op — computed in
 // fp32, rounded to fp16 before the next op reads it.  Here every product / sum / difference is one __fmul_rn /
@@ -32,6 +34,7 @@
 // source.  It stages them into shared memory with coalesced 16-byte loads (4-byte ones when the source is only 4-byte
 // aligned; blocks are mostly not 4-byte multiples, so per-thread loads from global would be unaligned), then each thread
 // decodes 8 consecutive outputs — always inside one sub-block — and writes them as one 16-byte vector.
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -229,10 +232,150 @@ void launch(const void* blocks, long long n, void* out, cudaStream_t s) {
   gguf_dequant_kernel<TYPE><<<(unsigned)grid, kThreads, 0, s>>>((const uint8_t*)blocks, n, (__half*)out, vec16);
 }
 
+// ---- expansion to bf16 in the engine layout (svr2_weight_expand_bf16): the weights a compressed-resident DiT keeps
+// in their storage format, decoded per transformer block into a staging slot.  The bf16 written equals what the
+// load-time path builds (svr2_gguf_dequant_f16, then torch's cast to bfloat16): the fp16 value of the block function
+// is rounded to bf16 (nearest even) in the same thread, no fp16 temporary is written.  The same CTA shape as above;
+// rows of the source may land in interleaved row groups of the destination (the SwiGLU [gate ; in] tiles).
+enum StorageFormat : int { kF16 = 2, kF8E4M3 = 3, kGgmlBase = 16 };   // svr2_tensor_desc.dtype codes
+
+constexpr bool is_ggml(int format) { return format >= kGgmlBase; }
+constexpr int fmt_block_elems(int format) { return is_ggml(format) ? block_elems(format - kGgmlBase) : 1; }
+constexpr int fmt_block_bytes(int format) {
+  return is_ggml(format) ? block_bytes(format - kGgmlBase) : (format == kF16 ? 2 : 1);
+}
+
+// float8_e4m3fn -> bf16 bits: every finite value is exact (3 mantissa bits, exponents 2^-9 .. 2^8); S.1111.111 is NaN
+__device__ __forceinline__ unsigned short e4m3_to_bf16(uint8_t b) {
+  const unsigned sign = (unsigned)(b & 0x80) << 8;
+  const int e = (b >> 3) & 15, m = b & 7;
+  if ((b & 0x7F) == 0x7F) return 0x7FC0;
+  if (e == 0) return (unsigned short)(sign | (__float_as_uint(__fmul_rn((float)m, 0x1p-9f)) >> 16));
+  return (unsigned short)(sign | ((unsigned)(e + 120) << 7) | ((unsigned)m << 4));
+}
+__device__ __forceinline__ unsigned short f32_to_bf16(float x) { return __bfloat16_as_ushort(__float2bfloat16_rn(x)); }
+
+template <int FORMAT>
+__global__ void __launch_bounds__(kThreads) weight_expand_kernel(const uint8_t* __restrict__ src, unsigned n_elem,
+                                                                 unsigned cols, unsigned short* __restrict__ dst,
+                                                                 unsigned row_group, unsigned group_stride,
+                                                                 unsigned row_offset, int vec16) {
+  constexpr int BE = fmt_block_elems(FORMAT), BB = fmt_block_bytes(FORMAT);
+  constexpr int kCtaBytes = kElemsPerCta / BE * BB;
+  static_assert(kCtaBytes % 16 == 0, "CTA byte range must keep the source alignment");
+  __shared__ __align__(16) uint8_t s[kCtaBytes];
+  const unsigned e_cta = blockIdx.x * (unsigned)kElemsPerCta;
+  const long long byte0 = (long long)(e_cta / BE) * BB;
+  const int nbytes = (int)min((long long)kCtaBytes, (long long)(n_elem / BE) * BB - byte0);
+  const uint8_t* g = src + byte0;
+  int done;
+  if (vec16) {
+    const int n16 = nbytes >> 4;
+    for (int i = threadIdx.x; i < n16; i += kThreads)
+      reinterpret_cast<uint4*>(s)[i] = __ldg(reinterpret_cast<const uint4*>(g) + i);
+    done = n16 << 4;
+  } else {
+    const int n4 = nbytes >> 2;
+    for (int i = threadIdx.x; i < n4; i += kThreads)
+      reinterpret_cast<uint32_t*>(s)[i] = __ldg(reinterpret_cast<const uint32_t*>(g) + i);
+    done = n4 << 2;
+  }
+  for (int i = done + threadIdx.x; i < nbytes; i += kThreads) s[i] = g[i];   // the tail of the last CTA
+  __syncthreads();
+
+  const int l = threadIdx.x * 8;               // first output of this thread, relative to the CTA
+  const unsigned e0 = e_cta + l;
+  if (e0 >= n_elem) return;                    // n_elem is a multiple of 8: a thread's outputs are all in or all out
+  uint4 pack;
+  unsigned short* pb = reinterpret_cast<unsigned short*>(&pack);
+  if constexpr (FORMAT == kF8E4M3) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) pb[k] = e4m3_to_bf16(s[l + k]);
+  } else if constexpr (FORMAT == kF16) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      pb[k] = f32_to_bf16(__half2float(__ushort_as_half(reinterpret_cast<const unsigned short*>(s)[l + k])));
+  } else {
+    float v[8];
+    decode8<FORMAT - kGgmlBase>(s + (l / BE) * BB, l % BE, v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) pb[k] = f32_to_bf16(h(v[k]));
+  }
+  const unsigned r = e0 / cols, c = e0 - r * cols;     // cols is a multiple of 8: the 8 outputs share a row
+  const unsigned grp = r / row_group;
+  const long long dst_row = (long long)grp * group_stride + row_offset + (r - grp * row_group);
+  *reinterpret_cast<uint4*>(dst + dst_row * cols + c) = pack;
+}
+
+template <int FORMAT>
+void launch_expand(const void* src, int64_t rows, int64_t cols, void* dst, int64_t group, int64_t stride, int64_t offset,
+                   cudaStream_t s) {
+  const unsigned n = (unsigned)(rows * cols);
+  const unsigned grid = (n + kElemsPerCta - 1) / kElemsPerCta;
+  const int vec16 = ((uintptr_t)src & 15) == 0;
+  weight_expand_kernel<FORMAT><<<grid, kThreads, 0, s>>>((const uint8_t*)src, n, (unsigned)cols, (unsigned short*)dst,
+                                                         (unsigned)group, (unsigned)stride, (unsigned)offset, vec16);
+}
+
 }  // namespace
+
+bool weight_format_size(int format, int* block_elems_out, int* block_bytes_out) {
+  if (format != kF16 && format != kF8E4M3) {
+    int e = 0, b = 0;
+    if (format < kGgmlBase || !geometry(format - kGgmlBase, &e, &b)) return false;
+  }
+  *block_elems_out = fmt_block_elems(format);
+  *block_bytes_out = fmt_block_bytes(format);
+  return true;
+}
+
 }  // namespace svr2
 
 using namespace svr2;
+
+extern "C" int svr2_weight_expand_bf16(int format, const void* src, int64_t rows, int64_t cols, void* dst,
+                                       int64_t dst_row_group, int64_t dst_group_stride, int64_t dst_row_offset,
+                                       void* stream) {
+  int be = 0, bb = 0;
+  if (!weight_format_size(format, &be, &bb)) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "svr2_weight_expand_bf16: format %d is not fp16 (2), fp8_e4m3fn (3) or 16 + a GGML type "
+             "the engine dequantizes", format);
+    return set_error(SVR2_ERR_ARG, buf);
+  }
+  if (rows <= 0 || cols <= 0) return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: empty matrix");
+  if (cols % (be > 8 ? be : 8))
+    return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: cols must be a multiple of the block size and of 8");
+  if (dst_row_group <= 0 || rows % dst_row_group)
+    return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: dst_row_group must divide rows");
+  if (dst_row_offset < 0 || dst_row_offset + dst_row_group > dst_group_stride)
+    return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: a row group must fit its stride: "
+                                   "0 <= dst_row_offset, dst_row_offset + dst_row_group <= dst_group_stride");
+  if (rows / dst_row_group * dst_group_stride >= ((int64_t)1 << 31) / cols)
+    return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: matrix too large (2^31 destination elements)");
+  if (!src || !dst) return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: null matrix");
+  if ((uintptr_t)src % 4) return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: src must be 4-byte aligned");
+  if ((uintptr_t)dst % 16) return set_error(SVR2_ERR_ARG, "svr2_weight_expand_bf16: dst must be 16-byte aligned");
+  cudaStream_t s = (cudaStream_t)stream;
+#define EXPAND(F) launch_expand<F>(src, rows, cols, dst, dst_row_group, dst_group_stride, dst_row_offset, s); break
+  switch (format) {
+    case kF16: EXPAND(kF16);
+    case kF8E4M3: EXPAND(kF8E4M3);
+    case kGgmlBase + kQ4_0: EXPAND(kGgmlBase + kQ4_0);
+    case kGgmlBase + kQ4_1: EXPAND(kGgmlBase + kQ4_1);
+    case kGgmlBase + kQ5_0: EXPAND(kGgmlBase + kQ5_0);
+    case kGgmlBase + kQ5_1: EXPAND(kGgmlBase + kQ5_1);
+    case kGgmlBase + kQ8_0: EXPAND(kGgmlBase + kQ8_0);
+    case kGgmlBase + kQ2_K: EXPAND(kGgmlBase + kQ2_K);
+    case kGgmlBase + kQ3_K: EXPAND(kGgmlBase + kQ3_K);
+    case kGgmlBase + kQ4_K: EXPAND(kGgmlBase + kQ4_K);
+    case kGgmlBase + kQ5_K: EXPAND(kGgmlBase + kQ5_K);
+    case kGgmlBase + kQ6_K: EXPAND(kGgmlBase + kQ6_K);
+    default: EXPAND(kGgmlBase + kBF16);
+  }
+#undef EXPAND
+  return check_launch("weight_expand");
+}
 
 extern "C" int svr2_gguf_type_size(int ggml_type, int* block_elems_out, int* block_bytes_out) {
   int e = 0, b = 0;

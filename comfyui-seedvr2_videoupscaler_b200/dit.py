@@ -19,7 +19,7 @@ from __future__ import annotations
 import math
 from dataclasses import dataclass
 from math import ceil
-from typing import Dict, List, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 
@@ -166,6 +166,92 @@ def rope_tables(freqs: torch.Tensor, variant: str, npos: int, size_rows: Dict[in
 
 
 # --------------------------------------------------------------------------
+# weights that stay compressed in device memory (resident="compressed")
+# --------------------------------------------------------------------------
+RESIDENT_MODES = ("expanded", "compressed")
+
+
+class MatrixPart(NamedTuple):
+    """One state-dict entry of a compressed block matrix and where svr2_weight_expand_bf16 puts its rows."""
+    key: str
+    format: int        # svr2_tensor_desc dtype code: lib.FMT_F16, lib.FMT_F8_E4M3 or lib.FMT_GGML + GGML type
+    rows: int
+    cols: int
+    row_group: int
+    group_stride: int
+    row_offset: int
+
+
+def storage_format(v) -> Optional[int]:
+    """Format code of a state-dict entry that can stay as stored: a GGUF-quantized entry (a ``load_gguf`` record or the
+    reference's ``GGUFTensor``) of a type the kernel decodes, or an fp8_e4m3fn tensor.  None for a dense entry."""
+    if weights._is_quantized(v):
+        return lib.FMT_GGML + int(v.tensor_type) if weights._known_block(int(v.tensor_type)) else None
+    if isinstance(v, torch.Tensor) and v.dtype == torch.float8_e4m3fn:
+        return lib.FMT_F8_E4M3
+    return None
+
+
+def _matrix_parts(sd, keys, swiglu: bool) -> Optional[List[MatrixPart]]:
+    entries = [sd[k] for k in keys]
+    fmts = [storage_format(v) for v in entries]
+    if all(f is None for f in fmts):
+        return None
+    parts = []
+    for j, (k, v, f) in enumerate(zip(keys, entries, fmts)):
+        if f is None:      # the dense half of a SwiGLU pair whose other half is compressed: fp16 expands to the same bf16
+            if not (isinstance(v, torch.Tensor) and v.dtype == torch.float16):
+                return None
+            f = lib.FMT_F16
+        shape = tuple(int(n) for n in (v.tensor_shape if weights._is_quantized(v) else v.shape))
+        block = weights.gguf_type_size(f - lib.FMT_GGML)[0] if f >= lib.FMT_GGML else 1
+        if len(shape) != 2 or shape[1] % max(block, 8):
+            return None
+        rows, cols = shape
+        if swiglu and (rows % 128 or (j and (rows, cols) != (parts[0].rows, parts[0].cols))):
+            return None
+        parts.append(MatrixPart(k, f, rows, cols, *((128, 256, 128 * j) if swiglu else (rows, rows, 0))))
+    return parts
+
+
+def compressed_matrices(cfg: dict, sd) -> Dict[str, List[MatrixPart]]:
+    """What ``resident="compressed"`` keeps in its storage format: engine-layout matrix name -> its state-dict
+    entries.  Only the four matrices of a block's stream qualify (``attn.proj_qkv``, ``attn.proj_out``, the MLP input
+    and output weights: over 99 % of the bytes), and only when their entries are quantized or fp8; a SwiGLU input matrix
+    is its ``proj_in_gate`` and ``proj_in`` entries, interleaved per 128 rows by the expansion.  Layers whose video
+    and text streams share weights (``all``) are listed once, under the video name."""
+    out: Dict[str, List[MatrixPart]] = {}
+    swiglu = cfg["mlp"] == "swiglu"
+    for i in range(cfg["layers"]):
+        shared = i >= cfg["mm_layers"]
+        last = cfg["last_vid_only"] and i == cfg["layers"] - 1
+        for s in (("vid",) if shared else ("vid", "txt")):
+            key, p = ("all" if shared else s), f"blocks.{i}."
+            mats = {"qkv.w": [p + f"attn.proj_qkv.{key}.weight"], "out.w": [p + f"attn.proj_out.{key}.weight"]}
+            if not (last and s == "txt"):
+                mats["mlp_in.w"] = [p + f"mlp.{key}.proj_in_gate.weight", p + f"mlp.{key}.proj_in.weight"] if swiglu \
+                    else [p + f"mlp.{key}.proj_in.weight"]
+                mats["mlp_out.w"] = [p + f"mlp.{key}.proj_out.weight"]
+            for n, keys in mats.items():
+                parts = _matrix_parts(sd, keys, swiglu and n == "mlp_in.w")
+                if parts:
+                    out[f"{i}.{s}.{n}"] = parts
+    return out
+
+
+def slot_layout(cfg: dict, plan: Dict[str, List[MatrixPart]]) -> Tuple[List[Dict[str, int]], int]:
+    """(per layer: matrix name -> byte offset in the staging slot, slot bytes): a block's compressed matrices in bf16
+    one after the other, each rounded up to 256 bytes; the slot is the largest block (csrc/engine.cu plans the same)."""
+    offsets: List[Dict[str, int]] = [{} for _ in range(cfg["layers"])]
+    ends = [0] * cfg["layers"]
+    for name, parts in plan.items():
+        i = int(name.split(".", 1)[0])
+        offsets[i][name] = ends[i]
+        ends[i] += (sum(p.rows for p in parts) * parts[0].cols * 2 + 255) // 256 * 256
+    return offsets, max(ends, default=0)
+
+
+# --------------------------------------------------------------------------
 # the engine
 # --------------------------------------------------------------------------
 class NaDiTOutput:
@@ -176,12 +262,23 @@ class NaDiTOutput:
 class B200NaDiT(EngineModule):
     """Drop-in for the reference ``runner.dit`` (VideoDiffusionInfer model slot, infer.py:361-367): an ``nn.Module``
     whose weights are buffers in the kernels' layout (see ``module.EngineModule`` for the lifecycle it survives) and
-    which holds one ``FlashAttentionVarlen`` submodule, the class ``apply_model_specific_config`` looks for."""
+    which holds one ``FlashAttentionVarlen`` submodule, the class ``apply_model_specific_config`` looks for.
+
+    ``resident``: ``"expanded"`` (default) expands every weight to bf16 once, at load.  ``"compressed"`` keeps the
+    block matrices of a GGUF-quantized or fp8_e4m3fn state dict in their storage format in device memory
+    (``compressed_matrices``) and expands each block's matrices to bf16 into a staging slot of the workspace just before
+    the block runs: the GEMMs read the same bf16 bytes, so the output is bit-identical, the resident weights shrink to
+    about the checkpoint's size and every forward pays the expansion.  A dense checkpoint has nothing to keep
+    compressed and loads the same in both modes."""
 
     K_IN_PAD = 192  # 4*33 = 132 patch channels padded to 3 k-blocks of 64
 
-    def __init__(self, cfg: dict, state_dict: Dict[str, torch.Tensor], device="cuda", timestep: float = 1000.0):
+    def __init__(self, cfg: dict, state_dict: Dict[str, torch.Tensor], device="cuda", timestep: float = 1000.0,
+                 resident: str = "expanded"):
+        if resident not in RESIDENT_MODES:
+            raise ValueError(f"resident must be one of {RESIDENT_MODES}, got {resident!r}")
         super().__init__(device)
+        self.resident = resident
         lib.device_check()
         self.cfg = cfg
         self.timestep = timestep
@@ -198,6 +295,7 @@ class B200NaDiT(EngineModule):
     def _device_state_moved(self):
         if hasattr(self, "_layouts"):
             self._layouts.clear()      # window / RoPE tables live on the old device
+        self.__dict__.pop("_stage", None)
         self._drop_handle()
 
     # ---- native runtime (csrc/engine.cu): the same forward sequenced in C++ on a svr2_t handle ---------------
@@ -219,15 +317,16 @@ class B200NaDiT(EngineModule):
         if self.__dict__.get("_handle"):
             return self._handle
         cfg = self.cfg
-        mlp_hidden = (self.W["0.vid.mlp_in.w"].shape[0] // 2) if cfg["mlp"] == "swiglu" else self.W["0.vid.mlp_in.w"].shape[0]
         desc = lib.ModelDesc(variant=0 if cfg["variant"] == "3b" else 1, dim=cfg["dim"], heads=cfg["heads"],
                              layers=cfg["layers"], mm_layers=cfg["mm_layers"], txt_in_dim=cfg["txt_in_dim"],
                              in_ch=cfg["in_ch"], out_ch=cfg["out_ch"], mlp_kind=0 if cfg["mlp"] == "swiglu" else 1,
-                             mlp_hidden=mlp_hidden, out_norm=int(cfg["out_norm"]), last_vid_only=int(cfg["last_vid_only"]),
+                             mlp_hidden=self.mlp_hidden, out_norm=int(cfg["out_norm"]), last_vid_only=int(cfg["last_vid_only"]),
                              eps=cfg["eps"], timestep=self.timestep)
         h = lib.engine_create(desc, self.device.index if self.device.index is not None else torch.cuda.current_device())
         try:
             lib.engine_load(h, {k: self.W[k] for k in self.W.keys()}, copy=False)
+            if self._formats:
+                lib.engine_load(h, {k: self.C[k] for k in self.C.keys()}, copy=False, formats=self._formats)
             lib.engine_load(h, {k: self.M[k] for k in self.M.keys()}, copy=False)
             lib.engine_load(h, {f"{i}.rope_freqs": f for i, f in enumerate(self.rope_freqs)}, copy=True)
         except Exception:
@@ -246,11 +345,28 @@ class B200NaDiT(EngineModule):
     def _f(self, sd, key):
         return sd[key].to(self.device, torch.float32).contiguous()
 
+    def _stored_bytes(self, v) -> torch.Tensor:
+        """The bytes of a quantized or fp8 entry as stored, 1-D uint8 on the device (4-byte aligned for the kernel)."""
+        t = weights._raw_blocks(v) if weights._is_quantized(v) else v.contiguous().view(torch.uint8).reshape(-1)
+        t = t.to(self.device)
+        return t.clone() if t.data_ptr() % 4 else t
+
     def _load(self, sd):
-        sd = weights.dequantizing(sd, self.device)   # GGUF entries: dense fp16 on the device, one key at a time
         cfg, dev = self.cfg, self.device
+        plan = compressed_matrices(cfg, sd) if self.resident == "compressed" else {}
+        stored = sd
+        sd = weights.dequantizing(sd, self.device)   # GGUF entries: dense fp16 on the device, one key at a time
         d = cfg["dim"]
         W: Dict[str, torch.Tensor] = {}
+        C: Dict[str, torch.Tensor] = {}                      # compressed matrices: the bytes of their entries
+        formats: Dict[str, Tuple[int, Tuple[int, int]]] = {}  # their format codes and logical shapes
+
+        def keep_compressed(name):
+            parts = plan.get(name)
+            for part, suffix in zip(parts or (), ("",) if parts and len(parts) == 1 else (".gate", ".in")):
+                C[name + suffix] = self._stored_bytes(stored[part.key])
+                formats[name + suffix] = (part.format, (part.rows, part.cols))
+            return parts is not None
         w_in = sd["vid_in.proj.weight"].to(dev, torch.bfloat16)
         w_pad = torch.zeros(d, self.K_IN_PAD, device=dev, dtype=torch.bfloat16)
         w_pad[:, : w_in.shape[1]] = w_in
@@ -268,9 +384,13 @@ class B200NaDiT(EngineModule):
                     for n in ("qkv.w", "out.w", "out.b", "nq", "nk", "nqk", "mlp_in.w", "mlp_in.b", "mlp_out.w", "mlp_out.b"):
                         if f"{i}.vid.{n}" in W:
                             W[f"{i}.txt.{n}"] = W[f"{i}.vid.{n}"]
+                    for n in [k[len(f"{i}.vid."):] for k in C if k.startswith(f"{i}.vid.")]:
+                        C[f"{i}.txt.{n}"], formats[f"{i}.txt.{n}"] = C[f"{i}.vid.{n}"], formats[f"{i}.vid.{n}"]
                     continue
-                W[f"{i}.{s}.qkv.w"] = self._w(sd, p + f"attn.proj_qkv.{key}.weight")
-                W[f"{i}.{s}.out.w"] = self._w(sd, p + f"attn.proj_out.{key}.weight")
+                if not keep_compressed(f"{i}.{s}.qkv.w"):
+                    W[f"{i}.{s}.qkv.w"] = self._w(sd, p + f"attn.proj_qkv.{key}.weight")
+                if not keep_compressed(f"{i}.{s}.out.w"):
+                    W[f"{i}.{s}.out.w"] = self._w(sd, p + f"attn.proj_out.{key}.weight")
                 W[f"{i}.{s}.out.b"] = self._w(sd, p + f"attn.proj_out.{key}.bias")
                 W[f"{i}.{s}.nq"] = self._f(sd, p + f"attn.norm_q.{key}.weight")
                 W[f"{i}.{s}.nk"] = self._f(sd, p + f"attn.norm_k.{key}.weight")
@@ -278,18 +398,22 @@ class B200NaDiT(EngineModule):
                 if last and s == "txt":
                     continue
                 if cfg["mlp"] == "swiglu":
-                    g = sd[p + f"mlp.{key}.proj_in_gate.weight"].to(dev, torch.bfloat16)
-                    u = sd[p + f"mlp.{key}.proj_in.weight"].to(dev, torch.bfloat16)
-                    hid = g.shape[0]
-                    assert hid % 128 == 0
-                    # interleave 128-row groups: tile j of 256 rows = [gate_j ; in_j]  (EPI_SWIGLU)
-                    il = torch.stack([g.view(hid // 128, 128, d), u.view(hid // 128, 128, d)], 1)
-                    W[f"{i}.{s}.mlp_in.w"] = il.reshape(2 * hid, d).contiguous()
-                    W[f"{i}.{s}.mlp_out.w"] = self._w(sd, p + f"mlp.{key}.proj_out.weight")
+                    if not keep_compressed(f"{i}.{s}.mlp_in.w"):
+                        g = sd[p + f"mlp.{key}.proj_in_gate.weight"].to(dev, torch.bfloat16)
+                        u = sd[p + f"mlp.{key}.proj_in.weight"].to(dev, torch.bfloat16)
+                        hid = g.shape[0]
+                        assert hid % 128 == 0
+                        # interleave 128-row groups: tile j of 256 rows = [gate_j ; in_j]  (EPI_SWIGLU)
+                        il = torch.stack([g.view(hid // 128, 128, d), u.view(hid // 128, 128, d)], 1)
+                        W[f"{i}.{s}.mlp_in.w"] = il.reshape(2 * hid, d).contiguous()
+                    if not keep_compressed(f"{i}.{s}.mlp_out.w"):
+                        W[f"{i}.{s}.mlp_out.w"] = self._w(sd, p + f"mlp.{key}.proj_out.weight")
                 else:
-                    W[f"{i}.{s}.mlp_in.w"] = self._w(sd, p + f"mlp.{key}.proj_in.weight")
+                    if not keep_compressed(f"{i}.{s}.mlp_in.w"):
+                        W[f"{i}.{s}.mlp_in.w"] = self._w(sd, p + f"mlp.{key}.proj_in.weight")
                     W[f"{i}.{s}.mlp_in.b"] = self._w(sd, p + f"mlp.{key}.proj_in.bias")
-                    W[f"{i}.{s}.mlp_out.w"] = self._w(sd, p + f"mlp.{key}.proj_out.weight")
+                    if not keep_compressed(f"{i}.{s}.mlp_out.w"):
+                        W[f"{i}.{s}.mlp_out.w"] = self._w(sd, p + f"mlp.{key}.proj_out.weight")
                     W[f"{i}.{s}.mlp_out.b"] = self._w(sd, p + f"mlp.{key}.proj_out.bias")
             fr = sd.get(p + "attn.rope.rope.freqs")
             if fr is None:
@@ -302,6 +426,10 @@ class B200NaDiT(EngineModule):
                 fr = torch.zeros(nfreq, dtype=sd["vid_in.proj.weight"].dtype)
             self.rope_freqs.append(fr.detach().cpu())
         self.W = self._register("w", W)
+        self.C, self._formats, self._plan = self._register("c", C), formats, plan
+        self._slot_offsets, self.slot_bytes = slot_layout(cfg, plan)
+        self.mlp_hidden = plan["0.vid.mlp_in.w"][0].rows if "0.vid.mlp_in.w" in plan else \
+            W["0.vid.mlp_in.w"].shape[0] // (2 if cfg["mlp"] == "swiglu" else 1)
         # ---- time embedding (constant: t == 1000, SURVEY.md fact 2) and AdaSingle vectors
         half = 128
         f = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32) / half)
@@ -389,6 +517,7 @@ class B200NaDiT(EngineModule):
                      lib.ptr(ws), ws.numel(), lib.stream())
             n_l = cfg["layers"]
             lib.LAUNCHES += 15 * n_l - (3 if cfg["last_vid_only"] else 0) + 5 + (1 if cfg["out_norm"] else 0) - 1
+            lib.LAUNCHES += sum(len(parts) for parts in self._plan.values())     # one expansion per compressed entry
             return NaDiTOutput(out)
         layouts, tables = self._geometry(T, Hp, Wp, l)
         st = lib.stream()
@@ -412,7 +541,8 @@ class B200NaDiT(EngineModule):
             last = cfg["last_vid_only"] and i == cfg["layers"] - 1
             lay = layouts[i % 2]
             cos_t, sin_t = tables[i]
-            k = lambda s, n: W[f"{i}.{s}.{n}"]
+            Wb = self._expand_block(i)     # this block's compressed matrices, as bf16 in the staging tensor
+            k = lambda s, n: Wb[f"{i}.{s}.{n}"] if f"{i}.{s}.{n}" in Wb else W[f"{i}.{s}.{n}"]
             m = lambda n: M[f"{i}.{n}"]
             # ---- attention branch
             a_v = lib.rmsnorm_ada(x, m("vid.attn_scale"), m("vid.attn_shift"), mode=0, eps=cfg["eps"])
@@ -446,8 +576,8 @@ class B200NaDiT(EngineModule):
             h_t = lib.linear(o_t, k("txt", "out.w"), bias=k("txt", "out.b"),
                              gate=None if last else m("txt.attn_gate"), residual=t)
             # ---- MLP branch
-            x = self._mlp(i, "vid", h_v)
-            t = h_t if last else self._mlp(i, "txt", h_t)   # last layer: text output is unused downstream
+            x = self._mlp(i, "vid", h_v, k)
+            t = h_t if last else self._mlp(i, "txt", h_t, k)   # last layer: text output is unused downstream
             del h_v
 
         if cfg["out_norm"]:
@@ -459,13 +589,37 @@ class B200NaDiT(EngineModule):
         lib.call("svr2_unpatchify_bf16", lib.ptr(v64), v64.stride(0), lib.ptr(out), T, H, Wd, cfg["out_ch"], st)
         return NaDiTOutput(out)
 
-    def _mlp(self, i, s, h):
+    def _expand_block(self, i: int) -> Dict[str, torch.Tensor]:
+        """Block i's compressed matrices expanded to bf16 (svr2_weight_expand_bf16) into the staging tensor the module
+        keeps, by name; the stream orders this after the previous block's GEMMs, which read the same tensor."""
+        offsets = self._slot_offsets[i]
+        if not offsets:
+            return {}
+        stage = self.__dict__.get("_stage")
+        if stage is None:
+            stage = self.__dict__["_stage"] = torch.empty(self.slot_bytes // 2, device=self.device, dtype=torch.bfloat16)
+        out = {}
+        for name, off in offsets.items():
+            parts = self._plan[name]
+            cols = parts[0].cols
+            dst = stage[off // 2: off // 2 + sum(p.rows for p in parts) * cols].view(-1, cols)
+            for part, suffix in zip(parts, ("",) if len(parts) == 1 else (".gate", ".in")):
+                src = self.C[name + suffix]
+                lib.call("svr2_weight_expand_bf16", part.format, lib.ptr(src), part.rows, cols, lib.ptr(dst),
+                         part.row_group, part.group_stride, part.row_offset, lib.stream(),
+                         nbytes=float(src.numel() + 2 * part.rows * cols))
+            out[name] = dst
+            if i >= self.cfg["mm_layers"]:      # shared weights: the text stream reads the same bytes
+                out[name.replace(".vid.", ".txt.", 1)] = dst
+        return out
+
+    def _mlp(self, i, s, h, k):
         cfg, W, M = self.cfg, self.W, self.M
         mm = lib.rmsnorm_ada(h, M[f"{i}.{s}.mlp_scale"], M[f"{i}.{s}.mlp_shift"], mode=1, eps=cfg["eps"])
         if cfg["mlp"] == "swiglu":
-            z = lib.linear(mm, W[f"{i}.{s}.mlp_in.w"], epi=EPI_SWIGLU)
-            return lib.linear(z, W[f"{i}.{s}.mlp_out.w"], gate=M[f"{i}.{s}.mlp_gate"], residual=h)
-        z = lib.linear(mm, W[f"{i}.{s}.mlp_in.w"], bias=W[f"{i}.{s}.mlp_in.b"], epi=EPI_GELU)
-        return lib.linear(z, W[f"{i}.{s}.mlp_out.w"], bias=W[f"{i}.{s}.mlp_out.b"], gate=M[f"{i}.{s}.mlp_gate"],
+            z = lib.linear(mm, k(s, "mlp_in.w"), epi=EPI_SWIGLU)
+            return lib.linear(z, k(s, "mlp_out.w"), gate=M[f"{i}.{s}.mlp_gate"], residual=h)
+        z = lib.linear(mm, k(s, "mlp_in.w"), bias=W[f"{i}.{s}.mlp_in.b"], epi=EPI_GELU)
+        return lib.linear(z, k(s, "mlp_out.w"), bias=W[f"{i}.{s}.mlp_out.b"], gate=M[f"{i}.{s}.mlp_gate"],
                           residual=h)
 

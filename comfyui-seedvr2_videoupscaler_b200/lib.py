@@ -104,6 +104,7 @@ SIGNATURES = {
     "svr2_sr_condition_bf16": [_P, _P, _P, _P, _P, _P, c_int64, c_int, _P],
     "svr2_gguf_type_size": [c_int, POINTER(c_int), POINTER(c_int)],
     "svr2_gguf_dequant_f16": [c_int, _P, c_int64, _P, _P],
+    "svr2_weight_expand_bf16": [c_int, _P, c_int64, c_int64, _P, c_int64, c_int64, c_int64, _P],
 }
 
 _lib = None
@@ -349,13 +350,18 @@ def engine_create(desc: ModelDesc, device_index: int) -> c_void_p:
     return h
 
 
-def engine_load(handle: c_void_p, tensors: dict, copy: bool) -> None:
-    """tensors: engine-layout name -> torch tensor (CUDA tensors are borrowed when copy is False; host tensors need copy)."""
+FMT_F16, FMT_F8_E4M3, FMT_GGML = 2, 3, 16     # storage formats of a compressed matrix: svr2_tensor_desc.dtype codes
+
+
+def engine_load(handle: c_void_p, tensors: dict, copy: bool, formats: dict = None) -> None:
+    """tensors: engine-layout name -> torch tensor (CUDA tensors are borrowed when copy is False; host tensors need copy).
+    formats: name -> (dtype code, logical shape) of the tensors that are the raw bytes of a compressed matrix."""
     items = [(k, t.contiguous()) for k, t in tensors.items()]
     arr = (TensorDesc * len(items))()
     for d, (k, t) in zip(arr, items):
-        d.name, d.data, d.dtype, d.rank = k.encode(), t.data_ptr(), _TORCH_DT[t.dtype], max(t.ndim, 1)
-        for i, n in enumerate(t.shape if t.ndim else (1,)):
+        code, shape = formats[k] if formats else (_TORCH_DT[t.dtype], t.shape if t.ndim else (1,))
+        d.name, d.data, d.dtype, d.rank = k.encode(), t.data_ptr(), code, len(shape)
+        for i, n in enumerate(shape):
             d.shape[i] = n
     _check(load().svr2_load_weights(handle, arr, len(items), int(copy)), "svr2_load_weights")
     if copy:

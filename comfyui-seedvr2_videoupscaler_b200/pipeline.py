@@ -55,9 +55,9 @@ def pad_video_temporal(frames: torch.Tensor, count: int = 0, prepend: bool = Fal
 
 class SeedVR2Engine:
     def __init__(self, dit_cfg: dict, dit_sd: Dict[str, torch.Tensor], vae_sd: Dict[str, torch.Tensor],
-                 txt_embed: torch.Tensor, device="cuda"):
+                 txt_embed: torch.Tensor, device="cuda", dit_resident: str = "expanded"):
         self.device = torch.device(device)
-        self.dit = B200NaDiT(dit_cfg, dit_sd, device=device)
+        self.dit = B200NaDiT(dit_cfg, dit_sd, device=device, resident=dit_resident)
         self.vae = B200VideoVAE(vae_sd, device=device)
         self.txt = txt_embed.to(self.device, torch.bfloat16).contiguous()
 
@@ -426,11 +426,15 @@ def build_synthetic_engine(variant="3b", device="cuda", seed=1234, txt_len=58) -
     return eng
 
 
-def build_engine(dit_checkpoint: str, vae_checkpoint: str, txt_embed, device="cuda") -> SeedVR2Engine:
+def build_engine(dit_checkpoint: str, vae_checkpoint: str, txt_embed, device="cuda",
+                 dit_resident: str = "expanded") -> SeedVR2Engine:
     """Engine from checkpoint files: DiT ``seedvr2_ema_{3b,7b}_{fp16,fp8_e4m3fn}.safetensors`` or a GGUF file
     (``seedvr2_ema_{3b,7b}-Q4_K_M.gguf`` …, dequantised on the device while the engine loads it), VAE
     ``ema_vae_fp16.safetensors`` (``model_registry.py:40-75``) and the positive text embedding (``pos_emb.pt``,
-    ``generation_utils.py:load_text_embeddings``) given as a path or tensor."""
+    ``generation_utils.py:load_text_embeddings``) given as a path or tensor.  ``dit_resident="compressed"`` keeps the
+    block matrices of a GGUF or fp8 DiT in their storage format in device memory and expands them per block on every
+    forward (``B200NaDiT``): same output, the resident weights shrink to about the file's size, and the VAE's slice
+    planner gets the difference."""
     from . import weights
     if dit_checkpoint.lower().endswith(".gguf"):
         dit_sd = weights.load_gguf(dit_checkpoint)
@@ -441,4 +445,5 @@ def build_engine(dit_checkpoint: str, vae_checkpoint: str, txt_embed, device="cu
     txt = torch.load(txt_embed, map_location="cpu", weights_only=True) if isinstance(txt_embed, str) else txt_embed
     if txt.ndim == 3:
         txt = txt[0]
-    return SeedVR2Engine(cfg, dit_sd, vae_sd, txt, device=device)
+    mode = {} if dit_resident == "expanded" else {"dit_resident": dit_resident}    # the default builds the engine as before
+    return SeedVR2Engine(cfg, dit_sd, vae_sd, txt, device=device, **mode)

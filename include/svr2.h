@@ -72,16 +72,26 @@ typedef struct svr2_model_desc {
 typedef struct svr2_tensor_desc {
   const char* name;   /* engine-layout name, e.g. "12.vid.qkv.w", "12.vid.attn_scale", "12.rope_freqs", "vid_in.w" */
   const void* data;   /* host or device pointer */
-  int dtype;          /* 0 fp32, 1 bf16, 2 fp16 */
+  int dtype;          /* 0 fp32, 1 bf16, 2 fp16; a compressed matrix (below): 3 fp8_e4m3fn, 16 + t = blocks of GGML type t */
   int rank;
-  int64_t shape[5];
+  int64_t shape[5];   /* the logical shape, also of a compressed matrix (its byte length follows from the dtype) */
 } svr2_tensor_desc;
 int svr2_create(svr2_t** out, int device, const svr2_model_desc* desc);
 void svr2_destroy(svr2_t* engine);
 const char* svr2_engine_last_error(svr2_t* engine);
 /* Weights in the engine layout (what weights.py / B200NaDiT._load produce: K-major bf16 matrices, SwiGLU gate / in rows
  * interleaved per 128, AdaSingle vectors E[:,layer,g] + P folded to fp32, "<i>.rope_freqs" in the checkpoint dtype).
- * copy != 0: the engine copies (caller keeps ownership of the source); copy == 0: device pointers are borrowed. */
+ * copy != 0: the engine copies (caller keeps ownership of the source); copy == 0: device pointers are borrowed.
+ *
+ * Compressed matrices.  The four matrices of a transformer block's stream ("<i>.<vid|txt>.qkv.w", ".out.w", ".mlp_in.w",
+ * ".mlp_out.w") may instead be given in their checkpoint storage format, dtype 3 or 16 + t, [N, K] row-major with K a
+ * multiple of the block size and of 8: they stay in that format in device memory, and every forward expands the
+ * matrices of a block to bf16 (svr2_weight_expand_bf16) into one staging slot of the workspace just before the block
+ * runs.  The slot is the largest per-block sum of those matrices in bf16 (each rounded up to 256 bytes) and is part of
+ * svr2_workspace_bytes; without a compressed matrix it is 0 bytes.  A SwiGLU "<i>.<s>.mlp_in.w" is compressed as its two
+ * checkpoint halves, "<i>.<s>.mlp_in.w.gate" (proj_in_gate) and "<i>.<s>.mlp_in.w.in" (proj_in), each [hidden, K] with
+ * dtype 2, 3 or 16 + t, given in place of "<i>.<s>.mlp_in.w"; the expansion interleaves their rows per 128.  Two names
+ * of one block that point at the same bytes (shared video / text weights) are expanded once. */
 int svr2_load_weights(svr2_t* engine, const svr2_tensor_desc* tensors, size_t n, int copy);
 /* bytes of engine-owned workspace one forward of this geometry uses (T, H, W = latent frames / rows / columns) */
 size_t svr2_workspace_bytes(svr2_t* engine, int T, int H, int W, int txt_len);
@@ -392,6 +402,18 @@ int svr2_gguf_type_size(int ggml_type, int* block_elems, int* block_bytes);
  * Bit-exact with the reference's float16 block functions: each product / sum / difference computed in fp32 and rounded
  * to fp16 before the next reads it (no FMA); BF16 is widened to fp32 and rounded to fp16 (out of range: +-inf). */
 int svr2_gguf_dequant_f16(int ggml_type, const void* blocks, int64_t n_elements, void* out, void* stream);
+/* Weight matrix in a storage format -> bf16 in the engine layout, for weights that stay compressed in device memory
+ * and are expanded per forward.  format (the svr2_tensor_desc dtype codes): 2 fp16, 3 fp8_e4m3fn, 16 + t = blocks of
+ * GGML type t (the types above).  src: rows x cols values, row-major (device, 4-byte aligned); cols a multiple of the
+ * format's block size and of 8.  Source row r is written to row
+ *   (r / dst_row_group) * dst_group_stride + dst_row_offset + r % dst_row_group
+ * of dst (bf16, row length cols, 16-byte aligned); dst_row_group divides rows.  Identity: group = stride = rows,
+ * offset = 0.  The SwiGLU input matrix [gate_j ; in_j] per 128 rows: group 128, stride 256, offset 0 for proj_in_gate
+ * and 128 for proj_in.  GGML blocks are decoded as svr2_gguf_dequant_f16 decodes them and the fp16 value is rounded to
+ * bf16 (nearest even), fp16 likewise; every finite fp8_e4m3fn value is exact in bf16 and its NaN becomes a bf16 NaN:
+ * the result is what a cast to bf16 of the fp16 / fp8 tensor gives.  Algorithmic bytes: the source plus 2 per value. */
+int svr2_weight_expand_bf16(int format, const void* src, int64_t rows, int64_t cols, void* dst, int64_t dst_row_group,
+                            int64_t dst_group_stride, int64_t dst_row_offset, void* stream);
 
 #ifdef __cplusplus
 }
