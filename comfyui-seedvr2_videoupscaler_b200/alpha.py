@@ -17,7 +17,7 @@ import torch
 
 from . import lib
 
-_DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+_DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2, torch.uint8: 3}    # uint8: as preprocess reads it
 OUT_F32, OUT_RGBA, OUT_RESIZE = 0, 1, 2
 
 

@@ -10,7 +10,8 @@ meaning and value ranges — for the methods the engine ships:
   ``wavelet_adaptive_color_correction(content_feat, style_feat, debug=None)`` (``color_fix.py:772-872``)
 
 plus ``sample_to_image`` = ``optimized_sample_to_image_format`` + ``clamp(-1,1)*0.5+0.5``
-(``generation_phases.py:1322-1345``) and ``apply_color_correction`` = the method switch of
+(``generation_phases.py:1322-1345``), ``sample_to_image_u8`` (the same, then the CLI's 8-bit frames) and
+``apply_color_correction`` = the method switch of
 ``generation_phases.py:1299-1317``.  Tensors are ``[T, 3, H, W]`` in ``[-1, 1]`` on the GPU; results are bf16 (the
 pipeline's compute dtype).  Every op is a libsvr2.so kernel (``csrc/post.cu``, ``csrc/hsv.cu``); there is no torch
 fallback.  The switch accepts "none", "lab", "wavelet", "adain" and "wavelet_adaptive"; "hsv" still raises there and
@@ -167,6 +168,22 @@ def sample_to_image_rgba(sample: torch.Tensor, image: torch.Tensor) -> torch.Ten
     lib.call("svr2_sample_to_image_rgba_bf16", lib.ptr(x), lib.ptr(image), T, H * W, lib.stream(),
              nbytes=4.0 * x.numel())
     return image
+
+
+def sample_to_image_u8(sample: torch.Tensor, image_rgba: torch.Tensor = None) -> torch.Tensor:
+    """``sample_to_image`` followed by the reference CLI's ``(frames.float() * 255.0).astype(np.uint8)``
+    (``inference_cli.py:590, 763, 809``) in one pass: ``[T, 3, H, W]`` -> ``[T, H, W, 3]`` uint8.  With ``image_rgba``
+    (``[T, H, W, 4]`` bf16 whose channel 3 holds the alpha, as for ``sample_to_image_rgba``) -> ``[T, H, W, 4]`` uint8,
+    the alpha scaled by 255 and truncated without normalisation."""
+    x = _as_planes(sample)
+    T, _, H, W = x.shape
+    C = 3 if image_rgba is None else 4
+    if image_rgba is not None:
+        assert image_rgba.shape == (T, H, W, 4) and image_rgba.dtype == torch.bfloat16 and image_rgba.is_contiguous()
+    out = torch.empty(T, H, W, C, device=x.device, dtype=torch.uint8)
+    lib.call("svr2_sample_to_image_u8", lib.ptr(x), lib.ptr(image_rgba), lib.ptr(out), T, H * W, lib.stream(),
+             nbytes=3.0 * x.numel() + (3.0 * T * H * W if C == 4 else 0.0))
+    return out
 
 
 def apply_color_correction(sample: torch.Tensor, input_video: torch.Tensor, color_correction: str = "lab",

@@ -7,6 +7,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stdint.h>
 
 namespace svr2 {
 namespace {
@@ -62,6 +63,12 @@ template <>
 __device__ __forceinline__ float load_bf16_rounded<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 template <>
 __device__ __forceinline__ float load_bf16_rounded<__half>(const __half* p) { return rn(__half2float(*p)); }
+// 8-bit frames as the reference CLI reads them (inference_cli.py:613, 336-339; generation_phases.py:380-387):
+// fp32(u) / 255 correctly rounded, then fp16, then the bf16 compute dtype
+template <>
+__device__ __forceinline__ float load_bf16_rounded<uint8_t>(const uint8_t* p) {
+  return rn(__half2float(__float2half_rn(__fdiv_rn((float)*p, 255.0f))));
+}
 
 inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 inline int taps_for(int in_size, int out_size) {

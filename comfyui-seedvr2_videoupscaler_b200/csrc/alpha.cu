@@ -404,7 +404,8 @@ int launch_stats(const void* alpha, int dtype, int channels, long long n_alpha, 
   alpha_stats_kernel<T><<<grid, 256, 0, s>>>((const T*)alpha, channels, n_alpha, (const __nv_bfloat16*)rgb, n_rgb, hdr)
   if (dtype == 0) SVR2_STATS(float);
   else if (dtype == 1) SVR2_STATS(__nv_bfloat16);
-  else SVR2_STATS(__half);
+  else if (dtype == 2) SVR2_STATS(__half);
+  else SVR2_STATS(uint8_t);
 #undef SVR2_STATS
   alpha_finalize_kernel<<<1, 1, 0, s>>>(hdr, n_alpha, allow_twice);
   return check_launch("alpha_stats");
@@ -425,7 +426,8 @@ extern "C" int svr2_alpha_upscale(const void* alpha_src, int src_dtype, int src_
                                   int64_t scratch_bytes, void* stream) {
   if (frames <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: empty image");
   if (frames > 65535) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: at most 65535 frames per call");
-  if (src_dtype < 0 || src_dtype > 2) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: src_dtype 0 fp32 | 1 bf16 | 2 fp16");
+  if (src_dtype < 0 || src_dtype > 3)
+    return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: src_dtype 0 fp32 | 1 bf16 | 2 fp16 | 3 uint8");
   if (src_channels != 1 && src_channels != 4)
     return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: src_channels must be 1 (alpha plane) or 4 (RGBA frames)");
   if (out_kind < 0 || out_kind > 2) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: out_kind 0 | 1 | 2");
@@ -464,7 +466,8 @@ extern "C" int svr2_alpha_upscale(const void* alpha_src, int src_dtype, int src_
                                                xcount, xw, yfirst, ycount, yw)
   if (src_dtype == 0) SVR2_ARESIZE(float);
   else if (src_dtype == 1) SVR2_ARESIZE(__nv_bfloat16);
-  else SVR2_ARESIZE(__half);
+  else if (src_dtype == 2) SVR2_ARESIZE(__half);
+  else SVR2_ARESIZE(uint8_t);
 #undef SVR2_ARESIZE
   rc = check_launch("alpha_resize");
   if (rc || out_kind == 2) return rc;

@@ -7,6 +7,7 @@
 //   rgb_to_lab / lab_to_rgb color_fix.py:368-474  sRGB <-> CIELAB (D65), fp32
 //   histogram match        color_fix.py:477-521   exact rank mapping: radix sort (CUB) + scatter
 //   sample_to_image        generation_phases.py:1322-1345   t c h w -> t h w c, clamp, [-1,1] -> [0,1]
+//   sample_to_image_u8     + inference_cli.py:763           the same, then the CLI's * 255 -> uint8, in one pass
 //
 // Rounding points follow the reference's bf16 flow (every torch op on a bf16 tensor rounds once); the LAB
 // part runs in fp32 as the reference does (ensure_float32_precision, color_fix.py:299-301).
@@ -237,6 +238,62 @@ __global__ void __launch_bounds__(256) sample_to_image_kernel(const __nv_bfloat1
   }
 }
 
+// The CLI's 8-bit frames (inference_cli.py:590, 763, 809: (frames.float() * 255.0).astype(uint8)) straight from the
+// sample: the image value of sample_to_image_kernel, one fp32 product (no FMA), truncated.  Image values lie in [0, 1];
+// an alpha outside it saturates (NaN -> 0), where numpy's cast is undefined.
+__device__ __forceinline__ float image_value(float s) {
+  const float v = fminf(fmaxf(s, -1.f), 1.f);
+  return rn(rn(v * 0.5f) + 0.5f);
+}
+__device__ __forceinline__ uint32_t to_byte(float x) {
+  return __float2uint_rz(fminf(fmaxf(__fmul_rn(x, 255.0f), 0.f), 255.f));
+}
+
+// [T,3,hw] bf16 (+ channel 3 of an RGBA bf16 image [T,hw,4] when C == 4) -> [T,hw,C] uint8, one pixel per thread
+template <int C>
+__global__ void __launch_bounds__(256) sample_to_image_u8_kernel(const __nv_bfloat16* __restrict__ in,
+                                                                 const __nv_bfloat16* __restrict__ rgba,
+                                                                 uint8_t* __restrict__ out, long long hw,
+                                                                 long long total) {
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const long long t = i / hw, px = i - t * hw;
+    const __nv_bfloat16* p = in + t * 3 * hw + px;
+    uint8_t* q = out + i * C;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) q[c] = (uint8_t)to_byte(image_value(bf2f(p[c * hw])));
+    if (C == 4) q[3] = (uint8_t)to_byte(bf2f(rgba[i * 4 + 3]));
+  }
+}
+
+// The same for hw % 4 == 0 and aligned buffers: four pixels per thread, 8-byte loads per channel plane, the 4*C output
+// bytes stored as C 32-bit words
+template <int C>
+__global__ void __launch_bounds__(256) sample_to_image_u8_x4_kernel(const uint2* __restrict__ in,
+                                                                    const __nv_bfloat16* __restrict__ rgba,
+                                                                    uint32_t* __restrict__ out, long long hw4,
+                                                                    long long total4) {
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total4; i += (long long)gridDim.x * 256) {
+    const long long t = i / hw4, g = i - t * hw4;
+    const uint2* p = in + t * 3 * hw4 + g;
+    uint32_t b[4 * C];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const uint2 v = p[c * hw4];
+      const uint32_t w[4] = {v.x << 16, v.x & 0xffff0000u, v.y << 16, v.y & 0xffff0000u};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) b[k * C + c] = to_byte(image_value(__uint_as_float(w[k])));
+    }
+    if (C == 4) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) b[k * C + 3] = to_byte(bf2f(rgba[(i * 4 + k) * 4 + 3]));
+    }
+    uint32_t* q = out + i * C;
+#pragma unroll
+    for (int j = 0; j < C; ++j)
+      q[j] = b[4 * j] | (b[4 * j + 1] << 8) | (b[4 * j + 2] << 16) | (b[4 * j + 3] << 24);
+  }
+}
+
 // Temporal-overlap cross-fade (blend_overlapping_frames, generation_utils.py:284-312):
 // out = rn(rn(prev * w_prev[f]) + rn(cur * w_cur[f])), frames of `frame_elems` bf16 values, 8 per thread
 __global__ void __launch_bounds__(256) blend_overlap_kernel(const uint4* __restrict__ prev, const uint4* __restrict__ cur,
@@ -449,6 +506,32 @@ extern "C" int svr2_sample_to_image_bf16(const void* sample, void* image, int fr
   sample_to_image_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)sample,
                                                                             (__nv_bfloat16*)image, hw, total);
   return check_launch("sample_to_image");
+}
+
+extern "C" int svr2_sample_to_image_u8(const void* sample, const void* alpha_rgba, void* image, int frames, int64_t hw,
+                                       void* stream) {
+  if (frames <= 0 || hw <= 0) return set_error(SVR2_ERR_ARG, "svr2_sample_to_image_u8: empty input");
+  if (!sample || !image) return set_error(SVR2_ERR_ARG, "svr2_sample_to_image_u8: null pointer");
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long total = (long long)frames * hw;
+  const __nv_bfloat16* a = (const __nv_bfloat16*)alpha_rgba;
+  const bool vec = hw % 4 == 0 && ((uintptr_t)sample % 8) == 0 && ((uintptr_t)image % (alpha_rgba ? 16 : 4)) == 0;
+  if (vec) {
+    const long long total4 = total / 4;
+    if (alpha_rgba)
+      sample_to_image_u8_x4_kernel<4><<<grid_for(total4), 256, 0, s>>>((const uint2*)sample, a, (uint32_t*)image,
+                                                                        hw / 4, total4);
+    else
+      sample_to_image_u8_x4_kernel<3><<<grid_for(total4), 256, 0, s>>>((const uint2*)sample, a, (uint32_t*)image,
+                                                                        hw / 4, total4);
+  } else if (alpha_rgba) {
+    sample_to_image_u8_kernel<4><<<grid_for(total), 256, 0, s>>>((const __nv_bfloat16*)sample, a, (uint8_t*)image, hw,
+                                                                  total);
+  } else {
+    sample_to_image_u8_kernel<3><<<grid_for(total), 256, 0, s>>>((const __nv_bfloat16*)sample, a, (uint8_t*)image, hw,
+                                                                  total);
+  }
+  return check_launch("sample_to_image_u8");
 }
 
 extern "C" int svr2_blend_overlap_bf16(const void* prev_tail, const void* cur_head, void* out, const float* w_prev,

@@ -118,7 +118,8 @@ extern "C" int svr2_resize_bicubic_aa_bf16(const void* in, int in_dtype, int cha
   if (in_dtype == 0) SVR2_RESIZE(float);
   else if (in_dtype == 1) SVR2_RESIZE(__nv_bfloat16);
   else if (in_dtype == 2) SVR2_RESIZE(__half);
-  else return set_error(SVR2_ERR_ARG, "svr2_resize: in_dtype 0 fp32 | 1 bf16 | 2 fp16");
+  else if (in_dtype == 3) SVR2_RESIZE(uint8_t);
+  else return set_error(SVR2_ERR_ARG, "svr2_resize: in_dtype 0 fp32 | 1 bf16 | 2 fp16 | 3 uint8");
 #undef SVR2_RESIZE
   return check_launch("resize_bicubic_aa");
 }

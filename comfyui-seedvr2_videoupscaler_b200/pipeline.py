@@ -11,11 +11,13 @@ correction against the input clip (``generation_phases.py:1249-1319``), [0,1] im
 RGBA clip keeps its alpha: edge-guided upscaling against the decoded RGB before colour correction (:1142-1217,
 ``alpha.py``).  ``input_noise_scale`` / ``latent_noise_scale`` blend noise into the encoder's input and the DiT's
 condition (:415-431, 679-704, ``noise.py``); ``upscale_video`` also takes the batch options ``uniform_batch_size`` and
-``prepend_frames`` (:95-101, 360-378, 949-958, 1388-1397).
+``prepend_frames`` (:95-101, 360-378, 949-958, 1388-1397).  ``stream_video`` runs the same batch loop over videos of
+any length, read in chunks and handed back to the host slice by slice (uint8 as the CLI writes frames, or bf16), with
+device memory independent of the length.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict, Iterator, Optional, Tuple
 
 import torch
 
@@ -155,21 +157,26 @@ class SeedVR2Engine:
 
     @staticmethod
     def finish_clip(sample: torch.Tensor, style: torch.Tensor, src: Optional[torch.Tensor] = None,
-                    color_correction: str = "none") -> torch.Tensor:
+                    color_correction: str = "none", out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
         """Phase 4 for one clip (or slice): optional colour correction, [0,1] image format (T,H,W,3).  ``src``: the
         input RGBA frames (T,h,w,4) of these output frames; their alpha is upscaled against the decoded sample before
-        the colour correction (which stays RGB-only) and becomes channel 3 of a (T,H,W,4) image."""
+        the colour correction (which stays RGB-only) and becomes channel 3 of a (T,H,W,4) image.
+        ``out_dtype=torch.uint8``: the reference CLI's 8-bit frames of that image, ``(image.float() * 255).to(uint8)``
+        with numpy's truncation, formatted in the same pass (``color_fix.sample_to_image_u8``)."""
+        if out_dtype not in (torch.bfloat16, torch.uint8):
+            raise ValueError(f"out_dtype must be torch.bfloat16 or torch.uint8, got {out_dtype}")
+        u8 = out_dtype == torch.uint8
         if src is None:
             if color_correction != "none":
                 sample = color_fix.apply_color_correction(sample, style, color_correction)
-            return color_fix.sample_to_image(sample)                # t h w c in [0,1]
+            return color_fix.sample_to_image_u8(sample) if u8 else color_fix.sample_to_image(sample)   # t h w c
         sample = sample.to(torch.bfloat16).contiguous()
         T, _, H, W = sample.shape
         image = torch.empty(T, H, W, 4, device=sample.device, dtype=torch.bfloat16)
         alpha.upscale_into_image(src, sample, image)
         if color_correction != "none":
             sample = color_fix.apply_color_correction(sample, style, color_correction)
-        return color_fix.sample_to_image_rgba(sample, image)
+        return color_fix.sample_to_image_u8(sample, image) if u8 else color_fix.sample_to_image_rgba(sample, image)
 
     @torch.no_grad()
     def clip_to_sample(self, frames: torch.Tensor, noise: Optional[torch.Tensor] = None, seed: int = 42,
@@ -244,20 +251,111 @@ class SeedVR2Engine:
         and its output trimmed back to the real frames (:95-101, 360-378, 949-958).  ``prepend_frames`` = p: p mirrored
         frames are put in front of the video and the first p output frames dropped, unless p is not smaller than the
         output (generation_utils.py:196-198, generation_phases.py:1388-1397).  A multi-GPU caller prepends once,
-        before sharding."""
+        before sharding.  Each slice is post-processed as soon as it is final (``final_slices``), so the device holds
+        the result and fewer than ``batch_size + temporal_overlap`` decoded frames; ``stream_video`` hands the slices
+        to the host instead."""
+        slices = [s for done in self._final_slices(frames, batch_size, temporal_overlap, seed, color_correction,
+                                                   resolution, max_resolution, keep_alpha, input_noise_scale,
+                                                   latent_noise_scale, uniform_batch_size, prepend_frames)
+                  for s in done]
+        out = torch.cat(slices, 0)
+        if 0 < prepend_frames < out.shape[0]:
+            out = out[prepend_frames:]
+        return out
+
+    @torch.no_grad()
+    def stream_video(self, frames, batch_size: int = 5, temporal_overlap: int = 0, seed: int = 42,
+                     color_correction: str = "none", resolution: Optional[int] = None, max_resolution: int = 0,
+                     keep_alpha: bool = False, input_noise_scale: float = 0.0, latent_noise_scale: float = 0.0,
+                     uniform_batch_size: bool = False, prepend_frames: int = 0,
+                     out_dtype: torch.dtype = torch.uint8) -> Iterator[Tuple[int, torch.Tensor]]:
+        """``upscale_video`` for videos of any length: device memory does not grow with the video.  ``frames``: one
+        (T,h,w,C) tensor or an iterable of (t,h,w,C) chunks of any sizes, on the host or the device (a decoder's
+        output, read only as far as the next batch needs; float in [0,1] or the reference CLI's uint8 RGB frames).
+        Yields ``(first_frame_index, frames)``, the output frames in order as soon as no later batch can change them,
+        each (t,H,W,C) in pinned host memory (torch's caching host allocator) that the caller owns.  C is 3, or 4
+        with ``keep_alpha`` and RGBA input.  ``out_dtype``: ``torch.uint8``, the CLI's 8-bit frames
+        (``(video.float() * 255.0).astype(np.uint8)`` of ``upscale_video``'s result), or ``torch.bfloat16``, that
+        result itself.  The other options are those of ``upscale_video``, with the same result frame for frame.
+
+        On the engine's one stream, every batch is enqueued first, then the cross-fade, phase 4 and the copy to the
+        host of the slices it made final, followed by an event; only then does the host wait for the copies enqueued
+        one batch earlier and yield them, so the consumer (an encoder, say) runs while the GPU computes the next
+        batch.  Held on the device: fewer than ``batch_size + temporal_overlap`` decoded frames and their styles
+        besides the batch in flight; with ``prepend_frames`` = p the first p output frames wait on the host until it
+        is known that more follow (the reference keeps all frames when p is not smaller than the output)."""
+        if out_dtype not in (torch.uint8, torch.bfloat16):
+            raise ValueError(f"out_dtype must be torch.uint8 or torch.bfloat16, got {out_dtype}")
+        cuda = self.device.type == "cuda"
+        p = prepend_frames
+        state = dict(seen=0, index=0)          # output frames so far (before the drop), frames yielded
+        kept = []                              # the first output frames while no more than p have come
+
+        def to_host(done):
+            host = []
+            for s in done:
+                h = torch.empty(s.shape, dtype=s.dtype, pin_memory=cuda)
+                h.copy_(s, non_blocking=cuda)
+                host.append(h)
+            ev = None
+            if cuda and host:
+                ev = torch.cuda.Event()
+                ev.record(torch.cuda.current_stream(self.device))
+            return host, ev
+
+        def release(host):
+            for h in host:
+                state["seen"] += h.shape[0]
+                if p > 0 and state["seen"] - h.shape[0] <= p:     # not yet known whether more than p frames come
+                    kept.append(h)
+                    if state["seen"] <= p:
+                        continue
+                    skip, pending = p, kept[:]          # more than p frames: the first p are dropped
+                    kept.clear()
+                    for k in pending:
+                        if skip < k.shape[0]:
+                            yield state["index"], k[skip:]
+                            state["index"] += k.shape[0] - skip
+                        skip = max(0, skip - k.shape[0])
+                else:
+                    yield state["index"], h
+                    state["index"] += h.shape[0]
+
+        prev = None
+        for done in self._final_slices(frames, batch_size, temporal_overlap, seed, color_correction, resolution,
+                                       max_resolution, keep_alpha, input_noise_scale, latent_noise_scale,
+                                       uniform_batch_size, prepend_frames, out_dtype):
+            cur = to_host(done)
+            del done
+            if prev is not None:
+                if prev[1] is not None:
+                    prev[1].synchronize()
+                yield from release(prev[0])
+            prev = cur
+        if prev is not None:
+            if prev[1] is not None:
+                prev[1].synchronize()
+            yield from release(prev[0])
+        for k in kept:                          # no more than p frames came: all are kept
+            yield state["index"], k
+            state["index"] += k.shape[0]
+
+    def _final_slices(self, frames, batch_size, temporal_overlap, seed, color_correction, resolution, max_resolution,
+                      keep_alpha, input_noise_scale, latent_noise_scale, uniform_batch_size, prepend_frames,
+                      out_dtype=torch.bfloat16):
+        """``final_slices`` over the engine's batches: per batch, the phase-4 images (on the device) it made final."""
         from . import shard
-        rgba = keep_alpha and frames.shape[-1] == 4
         input_noise_scale = gen_noise.check_scale("input_noise_scale", input_noise_scale)
         latent_noise_scale = gen_noise.check_scale("latent_noise_scale", latent_noise_scale)
         if prepend_frames < 0:
             raise ValueError(f"prepend_frames must be >= 0, got {prepend_frames}")
-        if prepend_frames > 0:
-            frames = pad_video_temporal(frames, count=prepend_frames, prepend=True)
+        source = FrameSource(frames, prepend_frames)
+        rgba = keep_alpha and source.channels == 4
         gen = gen_noise.input_generator(seed, self.device) if input_noise_scale > 0 else None
         noise_kw = dict(input_noise_scale=input_noise_scale, latent_noise_scale=latent_noise_scale, input_generator=gen)
 
         def clip(a, b):
-            batch = frames[a:b]
+            batch = source.take(a, b)
             if uniform_batch_size and b - a < batch_size:
                 batch = pad_video_temporal(batch, count=batch_size - (b - a))
             out = self.clip_to_sample(batch, seed=seed, resolution=resolution, max_resolution=max_resolution,
@@ -267,22 +365,26 @@ class SeedVR2Engine:
 
         def post(sample, style):
             style, src = style if rgba else (style, None)
-            return self.finish_clip(sample, style, src, color_correction=color_correction)
+            return self.finish_clip(sample, style, src, color_correction=color_correction, out_dtype=out_dtype)
 
-        out = run_batched(frames.shape[0], batch_size, temporal_overlap, clip, shard.blend_overlap, post)
-        if 0 < prepend_frames < out.shape[0]:
-            out = out[prepend_frames:]
-        return out
+        return final_slices(source, batch_size, temporal_overlap, clip, shard.blend_overlap, post)
 
+
+
+def _step(batch_size: int, temporal_overlap: int):
+    """(step, effective overlap) of generation_phases.py:271-289: overlap reset to 0 when it is not smaller than the
+    batch."""
+    step = batch_size - temporal_overlap if temporal_overlap > 0 else batch_size
+    if step <= 0:
+        step, temporal_overlap = batch_size, 0
+    return step, temporal_overlap
 
 
 def batch_ranges(total: int, batch_size: int, temporal_overlap: int = 0):
     """([start, end) per batch, effective overlap) of generation_phases.py:271-289, 344-358: step =
     batch_size - overlap (overlap reset to 0 when it is not smaller than the batch); a trailing batch that would hold
     nothing but overlap frames is dropped."""
-    step = batch_size - temporal_overlap if temporal_overlap > 0 else batch_size
-    if step <= 0:
-        step, temporal_overlap = batch_size, 0
+    step, temporal_overlap = _step(batch_size, temporal_overlap)
     out = []
     for idx in range(0, total, step):
         end = min(idx + batch_size, total)
@@ -292,23 +394,84 @@ def batch_ranges(total: int, batch_size: int, temporal_overlap: int = 0):
     return out, temporal_overlap
 
 
+class FrameSource:
+    """The frames of a video given as one (T,h,w,C) tensor or as an iterable of (t,h,w,C) chunks of any sizes (a
+    decoder's output, read as it comes).  ``fill(n)`` reads chunks until n frames are there or the input has ended;
+    ``take(a, b)`` returns frames [a, b) (one tensor, a view when they lie in one chunk) and lets go of every chunk
+    that ends at or before ``a``, so the frames held are those of the batch being read plus at most one chunk.
+    ``prepend`` = p puts the reference's p mirrored frames in front (``pad_video_temporal(video, p, prepend=True)``):
+    the p + 1 frames that takes are read ahead, or the whole video when it is shorter."""
+
+    def __init__(self, frames, prepend: int = 0):
+        self._chunks = iter((frames,) if isinstance(frames, torch.Tensor) else frames)
+        self._buf, self._start, self._end, self._done = [], 0, 0, False
+        self._read(max(1, prepend + 1))
+        self.channels = self._buf[0].shape[-1] if self._buf else 0
+        if prepend > 0 and self._end > 0:
+            head = self.take(0, min(prepend + 1, self._end))
+            self._buf.insert(0, pad_video_temporal(head, count=prepend, prepend=True)[:prepend])
+            self._end += prepend
+
+    def _read(self, n: int) -> None:
+        while self._end < n and not self._done:
+            c = next(self._chunks, None)
+            if c is None:
+                self._done = True
+            elif c.shape[0] > 0:
+                self._buf.append(c)
+                self._end += c.shape[0]
+
+    def fill(self, n: int) -> int:
+        """min(n, frames in the video), reading ahead as far as that needs."""
+        self._read(n)
+        return min(n, self._end)
+
+    def take(self, a: int, b: int) -> torch.Tensor:
+        self._read(b)
+        while self._buf and self._start + self._buf[0].shape[0] <= a:
+            self._start += self._buf.pop(0).shape[0]
+        if a < self._start or b > self._end:
+            raise IndexError(f"frames [{a}, {b}) are not held (held: [{self._start}, {self._end}))")
+        pieces, pos = [], self._start
+        for c in self._buf:
+            lo, hi = max(a, pos), min(b, pos + c.shape[0])
+            if lo < hi:
+                pieces.append(c[lo - pos:hi - pos])
+            pos += c.shape[0]
+            if pos >= b:
+                break
+        return pieces[0] if len(pieces) == 1 else torch.cat(pieces, 0)
+
+
 def _frames(x, sl: slice):
     return tuple(t[sl] for t in x) if isinstance(x, tuple) else x[sl]
 
 
-def run_batched(total: int, batch_size: int, temporal_overlap: int, clip_fn, blend_fn, post_fn) -> torch.Tensor:
-    """The reference's batch loop with the engine plugged in as callables: ``clip_fn(start, end) -> (sample, style)``
-    ((t,3,H,W) in [-1,1]; ``style`` may be a tuple of per-frame tensors, all sliced along frames alike),
-    ``blend_fn(prev_tail, cur_head)``, ``post_fn(sample, style) -> (t,H,W,C)``.  Decoded batches are
-    laid end to end; from the second batch on the first ``overlap`` frames are cross-faded into the tail already written
-    and dropped (generation_phases.py:969-1000), and phase 4 then post-processes every batch's slice against its own
-    input frames minus those overlap frames (:1249-1263)."""
-    ranges, overlap = batch_ranges(total, batch_size, temporal_overlap)
-    samples, styles = [], []
-    written = 0
-    for i, (a, b) in enumerate(ranges):
-        sample, style = clip_fn(a, b)
-        if i > 0 and overlap > 0 and overlap < sample.shape[0] and written >= overlap:
+def _own(x):
+    """Copies of trimmed views, so that the frames cut off are freed with their batch."""
+    return tuple(t.clone() for t in x) if isinstance(x, tuple) else x.clone()
+
+
+def final_slices(total, batch_size: int, temporal_overlap: int, clip_fn, blend_fn, post_fn):
+    """The batch loop of ``run_batched`` as a generator: after each batch, the list of ``post_fn(slice, style)`` of the
+    slices that became final with it, in order (often one, none while the overlap still reaches back into every held
+    slice, the rest once the input has ended).  A slice is final once at least ``overlap`` decoded frames follow it, as
+    no later cross-fade reaches further back.  ``total``: the frame count, or a ``FrameSource`` whose ``fill``
+    decides where the video ends (batches of ``batch_size`` frames are read ahead across chunk boundaries).
+
+    Held between batches: the slices not final yet, fewer than ``batch_size + overlap`` decoded frames, and their
+    styles (trimmed views are copied so that the overlap frames cut off them are not held as well)."""
+    step, overlap = _step(batch_size, temporal_overlap)
+    fill = total.fill if isinstance(total, FrameSource) else (lambda n: min(n, total))
+    samples, styles = [], []            # the slices not final yet, laid end to end, and their styles
+    written = held_from = 0             # decoded frames laid down so far; position of samples[0]
+    idx = 0
+    while True:
+        end = fill(idx + batch_size)
+        if end <= idx or (idx > 0 and end - idx <= overlap):
+            break
+        sample, style = clip_fn(idx, end)
+        if idx > 0 and overlap > 0 and overlap < sample.shape[0] and written >= overlap:
             # the tail lives in the previous batches' slices (it may span more than one when batches are short)
             tail = torch.cat(samples, 0)[-overlap:] if samples[-1].shape[0] < overlap else samples[-1][-overlap:]
             blended = blend_fn(tail.contiguous(), sample[:overlap].contiguous())
@@ -319,11 +482,34 @@ def run_batched(total: int, batch_size: int, temporal_overlap: int, clip_fn, ble
                 k -= n
                 if k == 0:
                     break
-            sample, style = sample[overlap:], _frames(style, slice(overlap, None))
+            sample, style = _own(sample[overlap:]), _own(_frames(style, slice(overlap, None)))
         samples.append(sample)
         styles.append(_frames(style, slice(None, sample.shape[0])))
         written += sample.shape[0]
-    return torch.cat([post_fn(s_, st_) for s_, st_ in zip(samples, styles)], 0)
+        idx += step
+        done = []
+        while samples and held_from + samples[0].shape[0] <= written - overlap:
+            held_from += samples[0].shape[0]
+            done.append(post_fn(samples.pop(0), styles.pop(0)))
+        yield done
+    if samples:
+        yield [post_fn(s_, st_) for s_, st_ in zip(samples, styles)]
+
+
+def iter_batched(total, batch_size: int, temporal_overlap: int, clip_fn, blend_fn, post_fn):
+    """``run_batched`` yielding each post-processed slice as soon as it is final (see ``final_slices``)."""
+    for done in final_slices(total, batch_size, temporal_overlap, clip_fn, blend_fn, post_fn):
+        yield from done
+
+
+def run_batched(total: int, batch_size: int, temporal_overlap: int, clip_fn, blend_fn, post_fn) -> torch.Tensor:
+    """The reference's batch loop with the engine plugged in as callables: ``clip_fn(start, end) -> (sample, style)``
+    ((t,3,H,W) in [-1,1]; ``style`` may be a tuple of per-frame tensors, all sliced along frames alike),
+    ``blend_fn(prev_tail, cur_head)``, ``post_fn(sample, style) -> (t,H,W,C)``.  Decoded batches are
+    laid end to end; from the second batch on the first ``overlap`` frames are cross-faded into the tail already written
+    and dropped (generation_phases.py:969-1000), and phase 4 then post-processes every batch's slice against its own
+    input frames minus those overlap frames (:1249-1263).  The concatenation of ``iter_batched``."""
+    return torch.cat(list(iter_batched(total, batch_size, temporal_overlap, clip_fn, blend_fn, post_fn)), 0)
 
 
 class GraphedClip:

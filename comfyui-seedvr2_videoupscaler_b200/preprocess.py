@@ -13,7 +13,8 @@ import torch
 
 from . import lib
 
-_DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+_DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2,
+           torch.uint8: 3}      # 8-bit RGB frames, read as the reference CLI reads them: fp16(u / 255)
 
 
 def resized_size(h: int, w: int, resolution: int, max_resolution: int = 0):
@@ -75,5 +76,5 @@ def prepare_video_transforms(resolution: int, max_resolution: int = 0, debug=Non
 
 
 def preprocess_frames(frames_thwc: torch.Tensor, resolution: int, max_resolution: int = 0) -> torch.Tensor:
-    """[T, h, w, C>=3] in [0,1] -> [3, T, Hp, Wp] bf16 in [-1,1]."""
+    """[T, h, w, C>=3] in [0,1] (or uint8 RGB, read as the CLI reads it) -> [3, T, Hp, Wp] bf16 in [-1,1]."""
     return VideoTransform(resolution, max_resolution).run(frames_thwc, channels_last=True)

@@ -312,6 +312,13 @@ int svr2_hsv_saturation_match_bf16(const void* content, const void* style, const
 /* final formatting (generation_phases.py:1322-1345): sample [frames,3,hw] bf16 -> image [frames,hw,3] bf16,
  * clamp(-1,1) * 0.5 + 0.5 */
 int svr2_sample_to_image_bf16(const void* sample, void* image, int frames, int64_t hw, void* stream);
+/* The same formatting straight to the reference CLI's 8-bit frames (inference_cli.py:590, 763, 809:
+ * (frames.float() * 255.0).astype(uint8)): image [frames,hw,C] uint8, each value the fp32 product of the bf16 image
+ * value and 255 (no FMA), truncated.  alpha_rgba == NULL: C = 3.  Otherwise C = 4 and channel 3 is channel 3 of the
+ * bf16 RGBA image alpha_rgba [frames,hw,4] (what svr2_alpha_upscale writes with out_kind 1), * 255 and truncated
+ * without normalisation; values outside [0, 255] saturate, NaN gives 0. */
+int svr2_sample_to_image_u8(const void* sample, const void* alpha_rgba, void* image, int frames, int64_t hw,
+                            void* stream);
 
 /* Temporal-overlap cross-fade of two neighbouring frame ranges (blend_overlapping_frames,
  * src/core/generation_utils.py:284-312): out[f] = bf16(bf16(prev[f] * w_prev[f]) + bf16(cur[f] * w_cur[f])); the
@@ -336,7 +343,8 @@ int svr2_tile_normalize_bf16(void* result, const void* count, int planes, int64_
 /* ---- Clip pre-processing (prepare_video_transforms, src/core/generation_utils.py:72-84; SURVEY.md §8(f) rank 3).
  * Antialiased bicubic resize (torchvision resize -> torch _upsample_bicubic2d_aa semantics, fp32 accumulation, result
  * rounded to bf16) of frames given as [T,h,w,cin] (channels_last != 0, first 3 channels) or [T,3,h,w]; in_dtype
- * 0 fp32 | 1 bf16 | 2 fp16, values rounded to bf16 on load (the pipeline's compute dtype).
+ * 0 fp32 | 1 bf16 | 2 fp16 | 3 uint8, values rounded to bf16 on load (the pipeline's compute dtype); a byte u loads as
+ * bf16(fp16(fp32(u) / 255)), the reference CLI's reading of 8-bit RGB frames (inference_cli.py:613, 336-339).
  *   finish == 0: out [T,3,H,W] bf16 (plain resize);
  *   finish != 0: out [3,T,Hp,Wp] bf16 = clamp(0,1) -> zero pad to multiples of 16 -> (x - 0.5) / 0.5 -> c t h w,
  *                Hp = ceil16(H), Wp = ceil16(W)  (what VideoDiffusionInfer.vae_encode consumes). */
@@ -352,7 +360,8 @@ int svr2_resize_bicubic_aa_bf16(const void* in, int in_dtype, int channels_last,
 int64_t svr2_alpha_upscale_scratch_bytes(int frames, int h, int w, int H, int W);
 /* Steps of :310-426 for `frames` frames:
  *   alpha_src [frames,h,w,src_channels] (src_channels 4: RGBA frames, 1: an alpha plane), the alpha is the last
- *     channel; src_dtype 0 fp32 | 1 bf16 | 2 fp16, rounded to bf16 on load (the clip in the compute dtype, :407-473);
+ *     channel; src_dtype 0 fp32 | 1 bf16 | 2 fp16 | 3 uint8 (loaded as the resize loads it), rounded to bf16 on load
+ *     (the clip in the compute dtype, :407-473);
  *   rgb_up [frames,3,H,W] bf16: the decoded sample before colour correction, the guide (:331-337);
  *   binary mask = (count(a < 0.1) + count(a > 0.9)) / numel > 0.95 over all frames (:319-324);
  *   guide = (rgb + 1) / 2 when min(rgb) < 0; Sobel edges of the guide (detect_edges_batch, :125-188, bit-exact);
