@@ -188,7 +188,7 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
 enum : int { KIND_BF16 = 0, KIND_SWIGLU = 1, KIND_F32 = 2, KIND_ROWSTAT = 3, KIND_PEXP = 4,
              KIND_QKV21 = 5, KIND_QKV10 = 6,
              KIND_BF16_RS = 7,
-             KIND_PEXP_STAT = 8 };   // KIND_PEXP that also emits per-slot (max score, sum of exponentials)   // KIND_BF16 with a per-row scale on the accumulator (its own instantiation: a runtime test in
+             KIND_PEXP_STAT = 8 };   // KIND_PEXP that also emits per-slot (0, sum of exponentials)   // KIND_BF16 with a per-row scale on the accumulator (its own instantiation: a runtime test in
                                    // the shared per-element loop cost the pixel-shuffle store 50 %)   // QKV projection + q/k RMSNorm + RoPE (21 / 10 frequencies per axis) + window scatter
 
 // KIND_BF16 epilogues start with bf16(acc + bias), and everything after it acts on that bf16 value: the MMA warpgroups
@@ -879,7 +879,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             __syncwarp();
           }
           if constexpr (KIND == KIND_PEXP_STAT) {
-            if (p.stat2) {     // this thread's row over this warp's columns of the tile: (max score, sum of exponentials)
+            if (p.stat2) {     // this thread's row over this warp's columns of the tile: (0, sum of exponentials)
               const int m = m_blk * BLOCK_M + row;
               if (m < p.M) {
                 const int slot = (N_COLS >= 64) ? n_blk * 2 + half : n_blk;
@@ -1241,7 +1241,7 @@ extern "C" int svr2_linear_bf16(const void* a, int64_t lda, const void* w, int64
 
 // svr2_linear_bf16 with the extras of the single-pass attention probabilities:
 //   rowscale (with SVR2_EPI_ROWSCALE): acc * rowscale[m] before the rest of the epilogue;
-//   stat_out (with SVR2_EPI_PEXP, N >= 256): float2 [M][ld_stat] = per (row, 128-column slot) (max acc*out_scale, sum of the
+//   stat_out (with SVR2_EPI_PEXP, N >= 256): float2 [M][ld_stat] = per (row, 128-column slot) (0, fp32 sum of the
 //     exponentials written), ld_stat >= 2 * ceil(N / 256);
 //   run_if: device flag — the launch does nothing unless *run_if != 0 (conditional fallback without a host sync).
 extern "C" int svr2_linear_ex_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, int M, int N, int K,
@@ -1297,7 +1297,7 @@ static int linear_impl(const void* a, int64_t lda, const void* w, int64_t ldw, i
     return set_error(SVR2_ERR_ARG, "EPI_ROWSTAT: ldc (float2 slots per row) must be >= svr2_rowstat_slots(N)");
   if ((p.epi & EPI_RESIDUAL) && !residual) return set_error(SVR2_ERR_ARG, "EPI_RESIDUAL without residual");
   if ((p.epi & EPI_ROWSCALE) && (!rowscale || bn < 128 || (p.epi & (EPI_SWIGLU | EPI_ROWSTAT | EPI_PEXP | EPI_F32))))
-    return set_error(SVR2_ERR_ARG, "EPI_ROWSCALE needs rowscale, a plain bf16 epilogue and N >= 128");
+    return set_error(SVR2_ERR_ARG, "EPI_ROWSCALE needs rowscale, a plain bf16 epilogue and N > 64 (128-column tiles)");
   if (stat_out && (!(p.epi & EPI_PEXP) || bn != 256 || ld_stat < 2 * (int64_t)p.num_n_tiles))
     return set_error(SVR2_ERR_ARG, "stat_out needs EPI_PEXP, N >= 256 and ld_stat >= 2 * ceil(N / 256)");
   p.rowscale = rowscale;

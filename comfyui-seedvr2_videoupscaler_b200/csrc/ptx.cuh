@@ -166,11 +166,14 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
 __device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 // exp2 on the FMA / ALU pipes (no MUFU): Cody-Waite split x = n + f with the round-to-nearest magic-number trick,
-// degree-4 polynomial for 2^f on [-0.5, 0.5] (relative error < 5e-5, far below the bf16 rounding of the probabilities it
-// feeds), exponent inserted with an integer add.  Valid for x in [-125, 127]; smaller x is clamped (result ~2^-125).
+// degree-4 polynomial for 2^f on [-0.5, 0.5] (relative error < 6e-5, far below the bf16 rounding of the probabilities it
+// feeds), exponent inserted with an integer add.  Accurate for x in [-125, 127].  x is clamped to [-125, 128] first:
+// below, the result is 2^-125 (ex2.approx.ftz gives 0 below -126); above, the integer add would carry into the sign bit
+// (NaN, -0 or a negative value for x >= 128.5).  At x = 128 the polynomial is exactly 1 and the add yields +inf, as
+// ex2.approx does, so an overflowing row sum stays visible to the caller's range check.
 // The MUFU pipe issues 16 ex2 per SM and clock — the bound of the exponent-heavy epilogues — while the FMA pipe idles.
 __device__ __forceinline__ float exp2_poly(float x) {
-  x = fmaxf(x, -125.0f);
+  x = fminf(fmaxf(x, -125.0f), 128.0f);
   const float t = x + 12582912.0f;                    // 1.5 * 2^23
   const float f = x - (t - 12582912.0f);
   float p = fmaf(f, 0.0096181291f, 0.0555041087f);

@@ -377,9 +377,9 @@ class B200VideoVAE(EngineModule):
         scale2 = (1.0 / (C ** 0.5)) * 1.4426950408889634
         # Default (n >= 256, n % 8 == 0): ONE Q K^T pass.  A 1/16-cost GEMM over every 16th key yields a reference
         # exponent per row; the full pass writes un-normalised bf16(exp2(s - ref)) and fp32 row sums; P~ @ V is divided
-        # by the row sum in its epilogue.  Exact (softmax is shift-invariant; bf16 rounding is relative) as long as the
-        # true row maximum is within 2^96 of the sampled one — checked on the device; the exact two-pass launches below
-        # are conditional on that flag and never ran in any test or benchmark.
+        # by the row sum in its epilogue.  Exact (softmax is shift-invariant; bf16 rounding is relative) as long as every
+        # row sum lies in (1e-30, 1e30) — checked on the device; the exact two-pass launches below are conditional on
+        # that flag.
         single = single_pass and n >= 256 and n % 8 == 0
         if single:
             k_sub_stride = 16

@@ -239,10 +239,10 @@ int svr2_rowstat_combine(const void* partial, int slots, int64_t ld, float* lse,
  *   1. reference exponent m^[m]: svr2_linear_bf16(q, every 16th key, SVR2_EPI_ROWSTAT) + svr2_rowstat_max — a 1/16-cost GEMM;
  *      any m^ within ~96 powers of two of the true row maximum is as good as the maximum itself;
  *   2. svr2_linear_ex_bf16(q, k, SVR2_EPI_PEXP, gate = m^, stat_out): un-normalised bf16(exp2(s - m^)) plus per-slot
- *      (max score, fp32 sum of the exponentials); svr2_pexp_stat_combine -> rowscale = 1 / sum and a device flag if some
- *      row's true maximum exceeded m^ by more than the safe margin (or the sum is not a positive finite number);
+ *      (0, fp32 sum of the exponentials); svr2_pexp_stat_combine -> rowscale = 1 / sum and a device flag if some row's
+ *      sum is not inside (1e-30, 1e30) (a score >= 128 powers of two above m^ makes it +inf);
  *   3. svr2_linear_ex_bf16(P~, V^T, SVR2_EPI_ROWSCALE, rowscale) = softmax(q k^T) v;
- *   4. the exact two-pass launches above with run_if = flag: no-ops unless step 2 raised it (never observed). */
+ *   4. the exact two-pass launches above with run_if = flag: no-ops unless step 2 raised it. */
 int svr2_linear_ex_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, int M, int N, int K, int epi_flags,
                         const void* bias, const float* gate, const void* residual, void* out, int64_t ldc, float out_scale,
                         const float* rowscale, void* stat_out, int64_t ld_stat, const int* run_if, void* stream);

@@ -1,5 +1,6 @@
 """Isolation timings of the epilogue-sensitive GEMM shapes of the 4K shard (short-K tiles, attention passes,
-shuffle store).  SVR2_AB_LIB=<path to another libsvr2.so> times a second build of the library for A/B runs."""
+shuffle store).  SVR2_AB_LIB=<path to another libsvr2.so> loads that build next to the in-tree one and times the two
+alternately in this process, ROUNDS times per case (default 3), so that both see the same clocks and neighbours."""
 import os, sys, importlib
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -7,24 +8,34 @@ sys.path.insert(0, ROOT)
 from svr2_import import load_package
 load_package()
 lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
+builds = [("tree", lib.load())]
 if os.environ.get("SVR2_AB_LIB"):
+    tree_path, lib._lib = lib.LIB_PATH, None
     lib.LIB_PATH = os.path.abspath(os.environ["SVR2_AB_LIB"])
+    builds.append(("ab", lib.load()))
+    lib.LIB_PATH = tree_path
+rounds = int(os.environ.get("ROUNDS", "3" if len(builds) > 1 else "1"))
 dev = "cuda"
 only = sys.argv[1] if len(sys.argv) > 1 else ""
 iters = int(os.environ.get("ITERS", "4"))
 flush = torch.empty(256 << 20, device=dev, dtype=torch.uint8)
 
 def timeit(fn, flops, name):
-    for _ in range(2): fn()
-    torch.cuda.synchronize()
-    tot = 0.0
-    for _ in range(iters):
-        flush.zero_()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(); fn(); e1.record(); torch.cuda.synchronize()
-        tot += e0.elapsed_time(e1)
-    ms = tot / iters
-    print(f"{name:40s} {ms:9.3f} ms  {flops / ms / 1e9:8.1f} TFLOP/s", flush=True)
+    for r in range(rounds):
+        for tag, handle in builds:
+            lib._lib = handle                   # lib.call dispatches through lib.load()
+            for _ in range(2): fn()
+            torch.cuda.synchronize()
+            tot = 0.0
+            for _ in range(iters):
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(); fn(); e1.record(); torch.cuda.synchronize()
+                tot += e0.elapsed_time(e1)
+            ms = tot / iters
+            label = f"{name} [{tag} {r}]" if len(builds) > 1 else name
+            print(f"{label:48s} {ms:9.3f} ms  {flops / ms / 1e9:8.1f} TFLOP/s", flush=True)
+    lib._lib = builds[0][1]
 
 def rnd(*s): return torch.randn(*s, device=dev, dtype=torch.bfloat16)
 
@@ -51,11 +62,18 @@ def mk_pexp():
     lse = torch.full((rows,), 12.0, device=dev)
     P = torch.empty(rows, n, device=dev, dtype=torch.bfloat16)
     return lambda: lib.linear(q, k[:n], epi=lib.EPI_PEXP, gate=lse, out=P, out_scale=0.0637)
+def mk_pexp_stat():                      # the single-pass probabilities: un-normalised exp2 + per-slot row sums
+    q, k = rnd(rows, C), rnd(n, C)
+    mhat = torch.full((rows,), 12.0, device=dev)
+    P = torch.empty(rows, n, device=dev, dtype=torch.bfloat16)
+    stat = torch.empty(rows, 2 * 2 * ((n + 255) // 256), device=dev)
+    return lambda: lib.linear(q, k, epi=lib.EPI_PEXP, gate=mhat, out=P, out_scale=0.0637, stat_out=stat)
 def mk_pv():
     P, vt = rnd(rows, n), rnd(C, n)
     return lambda: lib.linear(P, vt)
 cases.append(("attn_rowstat_e256 9472x129600x512", mk_rowstat, 2.0 * rows * n * C))
 cases.append(("attn_pexp_e512 9472x129600x512", mk_pexp, 2.0 * rows * n * C))
+cases.append(("attn_pexp_stat_e512 9472x129600x512", mk_pexp_stat, 2.0 * rows * n * C))
 cases.append(("attn_pv 9472x512x129600", mk_pv, 2.0 * rows * n * C))
 def mk_up():
     T, H, W, C = 2, 1080, 1920, 256
