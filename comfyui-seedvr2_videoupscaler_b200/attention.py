@@ -25,10 +25,6 @@ class FlashAttentionVarlen(nn.Module):
         self.attention_mode = attention_mode
         self.compute_dtype = compute_dtype
 
-    def run(self, q, k, v, cu_seqlens, max_seqlen, out=None, out_row_map=None, flops=0.0):
-        """The engine-internal call: window-ordered bf16 q/k/v, output scattered through ``out_row_map``."""
-        return lib.attn_varlen(q, k, v, cu_seqlens, max_seqlen, out=out, out_row_map=out_row_map, flops=flops)
-
     def forward(self, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, **kwargs):
         if q.shape[-1] != 128:
             raise lib.Svr2Error("b200 attention supports head_dim 128 only")

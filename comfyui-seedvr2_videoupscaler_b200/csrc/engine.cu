@@ -508,6 +508,26 @@ extern "C" size_t svr2_workspace_bytes(svr2_t* e, int T, int H, int W, int txt_l
   return make_plan(e->desc, T, H, W, txt_len, (int)max_total, (int)max_rows, fuse_qkv_ok(e, nfreq), e->slot_bytes).total;
 }
 
+// The tables svr2_dit_forward reads for one layer, built (on first use) by the same geometry() call
+extern "C" int svr2_dit_geometry(svr2_t* e, int T, int H, int W, int txt_len, int layer, svr2_dit_geometry_desc* out) {
+  if (!e || !out) return set_error(SVR2_ERR_ARG, "svr2_dit_geometry: null argument");
+  if (T <= 0 || H <= 0 || W <= 0 || (H & 1) || (W & 1) || txt_len <= 0)
+    return fail(e, SVR2_ERR_ARG, "svr2_dit_geometry: T, H, W > 0, H and W even, txt_len > 0");
+  int cur = 0;
+  cudaGetDevice(&cur);
+  if (cur != e->device) return fail(e, SVR2_ERR_ARG, "svr2_dit_geometry: the handle's device is not the current device");
+  if (e->desc.variant == 2) return fail(e, SVR2_ERR_ARG, "svr2_dit_geometry: the handle was created as a VAE (variant 2)");
+  if (layer < 0 || layer >= e->desc.layers) return fail(e, SVR2_ERR_ARG, "svr2_dit_geometry: layer outside [0, layers)");
+  const Geometry* g = geometry(e, T, H / 2, W / 2, txt_len);
+  if (!g) return fail(e, SVR2_ERR_ARG, "svr2_dit_geometry: geometry tables could not be built (missing '<i>.rope_freqs'?)");
+  const Layout& lay = g->lay[layer & 1];
+  const RopeTable& tab = g->tables[g->table_of_layer[layer]];
+  *out = svr2_dit_geometry_desc{lay.n_win, lay.total, lay.max_len, lay.n_txt_rows, g->nfreq, tab.rows,
+                                fuse_qkv_ok(e, g->nfreq) ? 1 : 0, lay.cu_seqlens, lay.row_src, lay.row_rope,
+                                lay.out_row_map, lay.tok_dst, lay.tok_rope, lay.txt_rows, tab.cos, tab.sin};
+  return SVR2_OK;
+}
+
 // One NaDiT forward: vid [T*H*W, in_ch] bf16 (latent pixels, channels last), txt [txt_len, txt_in_dim] bf16 ->
 // out [T*H*W, out_ch] bf16 (= NaDiTOutput.vid_sample).  Stream-ordered; the first call for a geometry builds and
 // uploads its index tables (synchronous copies) and may grow the workspace (cudaMalloc) — warm up before a graph capture.

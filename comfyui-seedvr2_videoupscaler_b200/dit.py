@@ -10,15 +10,14 @@ for b = 1, and replaces everything below it — ``NaMMSRTransformerBlock``
 ``SwiGLUMLP`` (``mlp.py:46-62``), ``NaPatchIn/Out`` (``patch/patch_v1.py:76-127``),
 ``TimeEmbedding`` (``embedding.py:25-62``) — with calls into libsvr2.so.
 
-Python here does only: weight re-layout at load, integer window/RoPE index
-bookkeeping (``window.py:28-83``, ``na.py:583-641``, ``rope.py:130-176``), buffer
-allocation and kernel sequencing.  No torch op touches activations on the hot path.
+Python here does only: weight re-layout at load, buffer allocation and kernel
+sequencing.  The window / RoPE index tables (``window.py:28-83``, ``na.py:583-641``,
+``rope.py:130-176``) are the native runtime's, read through ``svr2_dit_geometry``.
+No torch op touches activations on the hot path.
 """
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
-from math import ceil
 from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
@@ -43,126 +42,6 @@ def dit_config(variant: str = "3b", **over) -> dict:
         raise ValueError(variant)
     cfg.update(over)
     return cfg
-
-
-# --------------------------------------------------------------------------
-# window geometry (integer bookkeeping, host)
-# --------------------------------------------------------------------------
-def window_boxes(t: int, h: int, w: int, shifted: bool, num_windows=(4, 3, 3)) -> List[Tuple[int, ...]]:
-    """Window boxes in the reference's enumeration order (w-major, then h, then t):
-    make_720Pwindows_bysize / make_shifted_720Pwindows_bysize, dit_3b/window.py:28-83."""
-    rnt, rnh, rnw = num_windows
-    scale = math.sqrt((45 * 80) / (h * w))
-    rh, rw = round(h * scale), round(w * scale)
-    wh, ww = ceil(rh / rnh), ceil(rw / rnw)
-    wt = ceil(min(t, 30) / rnt)
-    if shifted:
-        st, sh, sw = (0.5 if wt < t else 0, 0.5 if wh < h else 0, 0.5 if ww < w else 0)
-        nt, nh, nw = ceil((t - st) / wt), ceil((h - sh) / wh), ceil((w - sw) / ww)
-        nt, nh, nw = (nt + 1 if st > 0 else 1, nh + 1 if sh > 0 else 1, nw + 1 if sw > 0 else 1)
-
-        def rng(i, s, win, ext):
-            return max(int((i - s) * win), 0), min(int((i - s + 1) * win), ext)
-    else:
-        st = sh = sw = 0
-        nt, nh, nw = ceil(t / wt), ceil(h / wh), ceil(w / ww)
-
-        def rng(i, s, win, ext):
-            return i * win, min((i + 1) * win, ext)
-    out = []
-    for iw in range(nw):
-        w0, w1 = rng(iw, sw, ww, w)
-        if w1 <= w0:
-            continue
-        for ih in range(nh):
-            h0, h1 = rng(ih, sh, wh, h)
-            if h1 <= h0:
-                continue
-            for it in range(nt):
-                t0, t1 = rng(it, st, wt, t)
-                if t1 <= t0:
-                    continue
-                out.append((t0, t1, h0, h1, w0, w1))
-    return out
-
-
-@dataclass
-class WindowLayout:
-    n_win: int
-    total: int            # L + n_win * l rows in window order
-    max_len: int
-    cu_seqlens: torch.Tensor   # int32 [n_win+1]
-    row_src: torch.Tensor      # int32 [total]   >=0 video token, <0 -(text idx + 1)
-    row_rope: torch.Tensor     # int32 [total,3] rows of the cos/sin tables (or -1)
-    out_row_map: torch.Tensor  # int32 [total]   video rows -> token idx, text rows -> L + w*l + j
-    attn_flops: float = 0.0    # sum over windows of 4 * len^2 * 128 (per head)
-    tok_dst: torch.Tensor = None    # int32 [L]    window-order row of every video token (inverse of row_src)
-    tok_rope: torch.Tensor = None   # int32 [L,3]  row_rope in token order
-    txt_rows: torch.Tensor = None   # int32 [n_win*l] window-order rows that hold text tokens
-
-
-def build_layout(T: int, Hp: int, Wp: int, l: int, shifted: bool, variant: str, device) -> Tuple[WindowLayout, dict]:
-    boxes = window_boxes(T, Hp, Wp, shifted)
-    L = T * Hp * Wp
-    grid = torch.arange(L, dtype=torch.int64).view(T, Hp, Wp)
-    src, rope, omap, lens = [], [], [], []
-    size_rows: Dict[int, int] = {}   # 7B: table offset for every distinct window-axis size
-    if variant == "7b":
-        off = 0
-        for b in boxes:
-            for n in (b[1] - b[0], b[3] - b[2], b[5] - b[4]):
-                if n not in size_rows:
-                    size_rows[n] = off
-                    off += n
-    tj = torch.arange(l, dtype=torch.int64)
-    for wi, (t0, t1, h0, h1, w0, w1) in enumerate(boxes):
-        sub = grid[t0:t1, h0:h1, w0:w1].reshape(-1)
-        tt, hh, ww_ = torch.meshgrid(torch.arange(t1 - t0), torch.arange(h1 - h0), torch.arange(w1 - w0),
-                                     indexing="ij")
-        if variant == "3b":   # rope.py:172-173: video (t + l, h, w) window-local; text (j, j, j)
-            r_v = torch.stack([tt.reshape(-1) + l, hh.reshape(-1), ww_.reshape(-1)], -1)
-            r_t = torch.stack([tj, tj, tj], -1)
-        else:                 # dit_7b/rope.py:73-111: video only
-            r_v = torch.stack([tt.reshape(-1) + size_rows[t1 - t0], hh.reshape(-1) + size_rows[h1 - h0],
-                               ww_.reshape(-1) + size_rows[w1 - w0]], -1)
-            r_t = torch.full((l, 3), -1, dtype=torch.int64)
-        src += [sub, -(tj + 1)]
-        rope += [r_v, r_t]
-        omap += [sub, L + wi * l + tj]
-        lens.append(sub.numel() + l)
-    lens_t = torch.tensor(lens, dtype=torch.int64)
-    cu = torch.zeros(len(lens) + 1, dtype=torch.int32)
-    cu[1:] = lens_t.cumsum(0).int()
-    src_all, rope_all = torch.cat(src), torch.cat(rope)
-    rows = torch.arange(src_all.numel())
-    is_vid = src_all >= 0
-    tok_dst = torch.empty(L, dtype=torch.int64)
-    tok_dst[src_all[is_vid]] = rows[is_vid]                  # the windows partition the tokens: a bijection
-    tok_rope = torch.empty(L, 3, dtype=torch.int64)
-    tok_rope[src_all[is_vid]] = rope_all[is_vid]
-    lay = WindowLayout(
-        n_win=len(boxes), total=int(lens_t.sum()), max_len=int(lens_t.max()),
-        cu_seqlens=cu.to(device), row_src=torch.cat(src).int().to(device),
-        row_rope=torch.cat(rope).int().contiguous().to(device), out_row_map=torch.cat(omap).int().to(device),
-        attn_flops=float((lens_t.double() ** 2).sum()) * 4 * 128,
-        tok_dst=tok_dst.int().to(device), tok_rope=tok_rope.int().contiguous().to(device),
-        txt_rows=rows[~is_vid].int().to(device))
-    return lay, size_rows
-
-
-def rope_tables(freqs: torch.Tensor, variant: str, npos: int, size_rows: Dict[int, int]):
-    """cos/sin tables [R, nfreq] fp32, evaluated the way rotary_embedding_torch does:
-    angle = pos.type(freqs.dtype) * freqs, cos/sin in that dtype (SURVEY.md §8 G4)."""
-    f = freqs.detach().cpu()
-    if variant == "3b":
-        pos = torch.arange(npos).type(f.dtype)
-    else:
-        rows = max((o + n for n, o in size_rows.items()), default=0)
-        pos = torch.zeros(rows, dtype=f.dtype)
-        for n, o in size_rows.items():
-            pos[o:o + n] = torch.linspace(-1, 1, steps=n).type(f.dtype)
-    ang = torch.einsum("p,f->pf", pos, f)
-    return ang.cos().float().contiguous(), ang.sin().float().contiguous()
 
 
 # --------------------------------------------------------------------------
@@ -282,19 +161,16 @@ class B200NaDiT(EngineModule):
         lib.device_check()
         self.cfg = cfg
         self.timestep = timestep
-        self._layouts: Dict[tuple, tuple] = {}
+        self._window_flops: Dict[tuple, List[float]] = {}
         self.attention = FlashAttentionVarlen()
         self._load(state_dict)
-        # the fused QKV epilogue needs 256-column tiles to be whole head pairs and one of the two shipped RoPE widths
-        # (the same rule as fuse_qkv_ok in csrc/engine.cu)
-        self.fuse_qkv = cfg["heads"] % 2 == 0 and self.rope_freqs[0].numel() in (21, 10)
         # forward sequenced by the native runtime (default) or by this module's Python loop (per-call profiling, tests
         # against the native runtime)
         self.native = True
 
     def _device_state_moved(self):
-        if hasattr(self, "_layouts"):
-            self._layouts.clear()      # window / RoPE tables live on the old device
+        if hasattr(self, "_window_flops"):
+            self._window_flops.clear()
         self.__dict__.pop("_stage", None)
         self._drop_handle()
 
@@ -313,7 +189,7 @@ class B200NaDiT(EngineModule):
 
     def native_handle(self):
         """svr2_t* that borrows this module's weight buffers (they stay under nn.Module lifecycle control) and owns
-        its workspace; rebuilt after a device move."""
+        its workspace and the window / RoPE tables both sequencings read; rebuilt after a device move."""
         if self.__dict__.get("_handle"):
             return self._handle
         cfg = self.cfg
@@ -460,27 +336,12 @@ class B200NaDiT(EngineModule):
         self.M = self._register("m", M)
         self.emb = None          # the raw time embedding is folded into M
 
-    # ---- geometry cache ----------------------------------------------------
-    def _geometry(self, T, Hp, Wp, l):
-        key = (T, Hp, Wp, l)
-        if key not in self._layouts:
-            variant = self.cfg["variant"]
-            lays, tabs = [], {}
-            for shifted in (False, True):
-                lay, size_rows = build_layout(T, Hp, Wp, l, shifted, variant, self.device)
-                lays.append((lay, size_rows))
-            tables = []
-            for i in range(self.cfg["layers"]):
-                lay, size_rows = lays[i % 2]
-                fr = self.rope_freqs[i]
-                tk = (i % 2, fr.dtype, tuple(fr.tolist()))
-                if tk not in tabs:
-                    npos = int(lay.row_rope.max().item()) + 1
-                    c, s = rope_tables(fr, variant, npos, size_rows)
-                    tabs[tk] = (c.to(self.device), s.to(self.device))
-                tables.append(tabs[tk])
-            self._layouts[key] = ([x[0] for x in lays], tables)
-        return self._layouts[key]
+    def _attn_flops(self, key: tuple, geo) -> List[float]:
+        """Per layout parity: Σ over the windows of 4·len²·128, the attention FLOPs of one head (profiler records)."""
+        if key not in self._window_flops:
+            cu = [lib.host_copy(g.cu_seqlens, (g.n_win + 1,), torch.int32) for g in geo[:2]]
+            self._window_flops[key] = [float((c.diff().double() ** 2).sum()) * 4 * 128 for c in cu]
+        return self._window_flops[key]
 
     # ---- forward -----------------------------------------------------------
     @torch.no_grad()
@@ -519,7 +380,9 @@ class B200NaDiT(EngineModule):
             lib.LAUNCHES += 15 * n_l - (3 if cfg["last_vid_only"] else 0) + 5 + (1 if cfg["out_norm"] else 0) - 1
             lib.LAUNCHES += sum(len(parts) for parts in self._plan.values())     # one expansion per compressed entry
             return NaDiTOutput(out)
-        layouts, tables = self._geometry(T, Hp, Wp, l)
+        # the tables svr2_dit_forward uses, layer by layer, from the handle
+        geo = [lib.dit_geometry(self.native_handle(), T, H, Wd, l, i) for i in range(cfg["layers"])]
+        attn_flops = self._attn_flops((T, H, Wd, l), geo)
         st = lib.stream()
 
         # stem
@@ -529,18 +392,16 @@ class B200NaDiT(EngineModule):
         t = lib.linear(txt, W["txt_in.w"], bias=W["txt_in.b"])
         del xp
 
-        max_total = max(lay.total for lay in layouts)
+        max_total = max(g.total for g in geo)
         qb = torch.empty(max_total, heads, 128, device=dev, dtype=torch.bfloat16)
         kb, vb = torch.empty_like(qb), torch.empty_like(qb)
-        max_rows = L + max(lay.n_win for lay in layouts) * l
+        max_rows = L + max(g.n_win for g in geo) * l
         o_all = torch.empty(max_rows, inner, device=dev, dtype=torch.bfloat16)
         o_t = torch.empty(l, inner, device=dev, dtype=torch.bfloat16)
-        nfreq = tables[0][0].shape[1]
 
         for i in range(cfg["layers"]):
             last = cfg["last_vid_only"] and i == cfg["layers"] - 1
-            lay = layouts[i % 2]
-            cos_t, sin_t = tables[i]
+            g = geo[i]
             Wb = self._expand_block(i)     # this block's compressed matrices, as bf16 in the staging tensor
             k = lambda s, n: Wb[f"{i}.{s}.{n}"] if f"{i}.{s}.{n}" in Wb else W[f"{i}.{s}.{n}"]
             m = lambda n: M[f"{i}.{n}"]
@@ -548,30 +409,29 @@ class B200NaDiT(EngineModule):
             a_v = lib.rmsnorm_ada(x, m("vid.attn_scale"), m("vid.attn_shift"), mode=0, eps=cfg["eps"])
             a_t = lib.rmsnorm_ada(t, m("txt.attn_scale"), m("txt.attn_shift"), mode=0, eps=cfg["eps"])
             qkv_t = lib.linear(a_t, k("txt", "qkv.w"))
-            q, kk, v = qb[: lay.total], kb[: lay.total], vb[: lay.total]
-            rope_args = (lib.ptr(cos_t), lib.ptr(sin_t), nfreq)
-            if self.fuse_qkv:
+            q, kk, v = qb[: g.total], kb[: g.total], vb[: g.total]
+            rope_args = (g.rope_cos, g.rope_sin, g.nfreq)
+            if g.fuse_qkv:
                 # video rows: q/k RMSNorm + RoPE + window scatter inside the QKV GEMM's epilogue; text rows (the same
                 # 58 rows appended to every window) by the row-subset form of the stand-alone kernel
                 lib.call("svr2_linear_qkv_rope_bf16", lib.ptr(a_v), a_v.stride(0), lib.ptr(k("vid", "qkv.w")), d, L, heads, d,
-                         lib.ptr(lay.tok_dst), lib.ptr(lay.tok_rope), *rope_args, lib.ptr(k("vid", "nqk")), cfg["eps"],
+                         g.tok_dst, g.tok_rope, *rope_args, lib.ptr(k("vid", "nqk")), cfg["eps"],
                          lib.ptr(q), lib.ptr(kk), lib.ptr(v), st, flops=2.0 * L * 3 * inner * d)
-                lib.call("svr2_qk_norm_rope_rows_bf16", None, lib.ptr(qkv_t), lib.ptr(lay.row_src), lib.ptr(lay.row_rope),
-                         *rope_args, lib.ptr(k("vid", "nq")), lib.ptr(k("vid", "nk")), lib.ptr(k("txt", "nq")),
-                         lib.ptr(k("txt", "nk")), cfg["eps"], lib.ptr(lay.txt_rows), lay.txt_rows.numel(), heads,
-                         lib.ptr(q), lib.ptr(kk), lib.ptr(v), st, nbytes=12.0 * lay.txt_rows.numel() * inner)
+                lib.call("svr2_qk_norm_rope_rows_bf16", None, lib.ptr(qkv_t), g.row_src, g.row_rope, *rope_args,
+                         lib.ptr(k("vid", "nq")), lib.ptr(k("vid", "nk")), lib.ptr(k("txt", "nq")), lib.ptr(k("txt", "nk")),
+                         cfg["eps"], g.txt_rows, g.n_txt_rows, heads, lib.ptr(q), lib.ptr(kk), lib.ptr(v), st,
+                         nbytes=12.0 * g.n_txt_rows * inner)
             else:
                 qkv_v = lib.linear(a_v, k("vid", "qkv.w"))
-                lib.call("svr2_qk_norm_rope_window_bf16", lib.ptr(qkv_v), lib.ptr(qkv_t), lib.ptr(lay.row_src),
-                         lib.ptr(lay.row_rope), *rope_args, lib.ptr(k("vid", "nq")),
-                         lib.ptr(k("vid", "nk")), lib.ptr(k("txt", "nq")), lib.ptr(k("txt", "nk")), cfg["eps"],
-                         lay.total, heads, lib.ptr(q), lib.ptr(kk), lib.ptr(v), st, nbytes=12.0 * lay.total * inner)
+                lib.call("svr2_qk_norm_rope_window_bf16", lib.ptr(qkv_v), lib.ptr(qkv_t), g.row_src, g.row_rope,
+                         *rope_args, lib.ptr(k("vid", "nq")), lib.ptr(k("vid", "nk")), lib.ptr(k("txt", "nq")),
+                         lib.ptr(k("txt", "nk")), cfg["eps"], g.total, heads, lib.ptr(q), lib.ptr(kk), lib.ptr(v), st,
+                         nbytes=12.0 * g.total * inner)
                 del qkv_v
             del a_v
-            o_view = o_all.view(-1, heads, 128)
-            self.attention.run(q, kk, v, lay.cu_seqlens, lay.max_len, out=o_view, out_row_map=lay.out_row_map,
-                               flops=lay.attn_flops * heads)
-            lib.call("svr2_txt_window_mean_bf16", lib.ptr(o_all[L:]), lib.ptr(o_t), lay.n_win, l, inner, st)
+            lib.call("svr2_attn_varlen_bf16", lib.ptr(q), lib.ptr(kk), lib.ptr(v), lib.ptr(o_all), g.cu_seqlens, g.n_win,
+                     g.total, heads, g.max_len, g.out_row_map, st, flops=attn_flops[i % 2] * heads)
+            lib.call("svr2_txt_window_mean_bf16", lib.ptr(o_all[L:]), lib.ptr(o_t), g.n_win, l, inner, st)
             h_v = lib.linear(o_all[:L], k("vid", "out.w"), bias=k("vid", "out.b"), gate=m("vid.attn_gate"), residual=x)
             h_t = lib.linear(o_t, k("txt", "out.w"), bias=k("txt", "out.b"),
                              gate=None if last else m("txt.attn_gate"), residual=t)

@@ -29,6 +29,13 @@ class TensorDesc(ctypes.Structure):
     _fields_ = [("name", ctypes.c_char_p), ("data", c_void_p), ("dtype", c_int), ("rank", c_int), ("shape", c_int64 * 5)]
 
 
+class DitGeometryDesc(ctypes.Structure):
+    """svr2_dit_geometry_desc (include/svr2.h)"""
+    _fields_ = [(n, c_int) for n in ("n_win", "total", "max_len", "n_txt_rows", "nfreq", "rope_rows", "fuse_qkv")] + \
+               [(n, c_void_p) for n in ("cu_seqlens", "row_src", "row_rope", "out_row_map", "tok_dst", "tok_rope",
+                                        "txt_rows", "rope_cos", "rope_sin")]
+
+
 # name -> argtypes; every function returns int (svr2_status) except svr2_last_error
 _P = c_void_p
 SIGNATURES = {
@@ -40,6 +47,7 @@ SIGNATURES = {
     "svr2_workspace_bytes": [_P, c_int, c_int, c_int, c_int],
     "svr2_dit_forward": [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P],
     "svr2_dit_forward_ws": [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
+    "svr2_dit_geometry": [_P, c_int, c_int, c_int, c_int, c_int, POINTER(DitGeometryDesc)],
     "svr2_vae_workspace_bytes": [_P, c_int, c_int, c_int, c_int, c_int],
     "svr2_vae_encode": [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
     "svr2_vae_decode": [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
@@ -372,3 +380,21 @@ def engine_load(handle: c_void_p, tensors: dict, copy: bool, formats: dict = Non
 def engine_destroy(handle) -> None:
     if handle:
         load().svr2_destroy(handle)
+
+
+def dit_geometry(handle: c_void_p, T: int, H: int, W: int, txt_len: int, layer: int) -> DitGeometryDesc:
+    """The window layout and RoPE table svr2_dit_forward uses in one layer (device pointers owned by the handle)."""
+    g = DitGeometryDesc()
+    _check(load().svr2_dit_geometry(handle, T, H, W, txt_len, layer, ctypes.byref(g)), "svr2_dit_geometry")
+    return g
+
+
+class _DeviceArray:
+    def __init__(self, address: int, shape, typestr: str):
+        self.__cuda_array_interface__ = {"data": (address, False), "shape": tuple(shape), "typestr": typestr, "version": 2}
+
+
+def host_copy(address: int, shape, dtype: torch.dtype) -> torch.Tensor:
+    """A host copy of device memory the library owns (int32 or fp32 elements, e.g. a svr2_dit_geometry table)."""
+    typestr = {torch.int32: "<i4", torch.float32: "<f4"}[dtype]
+    return torch.as_tensor(_DeviceArray(address, shape, typestr)).cpu()

@@ -103,6 +103,23 @@ int svr2_dit_forward(svr2_t* engine, const void* vid, const void* txt, int T, in
  * retains nothing, so hosts that pool device memory (PyTorch's allocator, a CUDA-graph capture) keep control of it */
 int svr2_dit_forward_ws(svr2_t* engine, const void* vid, const void* txt, int T, int H, int W, int txt_len, void* out,
                         void* workspace, size_t workspace_bytes, void* stream);
+/* The window layout and RoPE cos / sin table the forward of this geometry uses in `layer`, built on first use as the
+ * forward builds them (synchronous uploads).  The pointers are device memory the handle owns, valid until the next
+ * svr2_load_weights or svr2_destroy.  Layout rows are in window order: each window's video tokens, then the txt_len
+ * text tokens. */
+typedef struct svr2_dit_geometry_desc {
+  int n_win, total, max_len, n_txt_rows; /* the layer's layout: regular windows for an even layer, shifted for an odd one */
+  int nfreq, rope_rows, fuse_qkv;        /* the layer's table; fuse_qkv: the forward fuses q/k norm + RoPE into the QKV GEMM */
+  const int32_t* cu_seqlens;             /* [n_win + 1] */
+  const int32_t* row_src;                /* [total] video token, or -(text index + 1) */
+  const int32_t* row_rope;               /* [total, 3] table rows of the (t, h, w) rotations, -1: none */
+  const int32_t* out_row_map;            /* [total] attention output row: video token, or T*H/2*W/2 + window * txt_len + j */
+  const int32_t* tok_dst;                /* [T*H/2*W/2] the window-order row of every video token */
+  const int32_t* tok_rope;               /* [T*H/2*W/2, 3] row_rope in token order */
+  const int32_t* txt_rows;               /* [n_txt_rows] the window-order rows of text tokens */
+  const float *rope_cos, *rope_sin;      /* [rope_rows, nfreq] */
+} svr2_dit_geometry_desc;
+int svr2_dit_geometry(svr2_t* engine, int T, int H, int W, int txt_len, int layer, svr2_dit_geometry_desc* out);
 
 /* ---- Video VAE on a handle created with svr2_model_desc.variant == 2 (native host runtime csrc/vae_engine.cu).
  * Replaces VideoAutoencoderKLWrapper.encode / .decode (video_vae_v3/modules/attn_video_vae.py:1680-1698) incl. the

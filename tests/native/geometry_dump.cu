@@ -1,5 +1,5 @@
 // Test harness (CPU): the native runtime's geometry code (csrc/engine.cu) compiled with SVR2_HOST_TEST so that its
-// tables stay in host memory; dumps them as text for tests/test_native_geometry_cpu.py to compare with dit.py.
+// tables stay in host memory; dumps them as text for tests/test_native_geometry_cpu.py to compare with the oracle.
 // usage: geometry_dump T Hp Wp l is7 fdtype nfreq f0 f1 ... > out.txt
 #define SVR2_HOST_TEST 1
 #include "../../comfyui-seedvr2_videoupscaler_b200/csrc/engine.cu"
@@ -31,7 +31,7 @@ int main(int argc, char** argv) {
       for (int i = 0; i < n; ++i) printf(" %d", p[i]);
       printf("\n");
     };
-    dump("cu", L.cu_seqlens, L.n_win + 1);
+    dump("cu_seqlens", L.cu_seqlens, L.n_win + 1);
     dump("row_src", L.row_src, L.total);
     dump("row_rope", L.row_rope, L.total * 3);
     dump("out_row_map", L.out_row_map, L.total);

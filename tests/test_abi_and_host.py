@@ -1,5 +1,5 @@
 """CPU: the C-ABI library loads and exports every symbol include/svr2.h declares (no compute
-calls without a GPU); host-side integer logic (windows, layouts, padding, sharding)."""
+calls without a GPU); host-side integer logic (padding, sharding, batching)."""
 import importlib
 import os
 import re
@@ -52,65 +52,6 @@ def test_product_path_has_no_oracle_or_fallback():
             src = open(os.path.join(pk, fn)).read()
             assert "oracle" not in src.replace("oracle/", ""), f"{fn} must not import the oracle"
             assert "scaled_dot_product_attention" not in src and "F.conv3d" not in src
-
-
-@pytest.mark.parametrize("thw,counts", [((1, 32, 32), (4, 9)), ((5, 68, 120), (75, 90)), ((3, 135, 240), (243, 300)),
-                                        ((17, 135, 240), (324, 400)), ((2, 135, 240), (162, 200))])
-def test_window_counts_match_survey(pkg, thw, counts):
-    import importlib
-    dit = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.dit")
-    for shifted, n in zip((False, True), counts):
-        boxes = dit.window_boxes(*thw, shifted)
-        assert len(boxes) == n
-        assert boxes == dit_oracle.window_boxes(*thw, shifted)
-        # every token covered exactly once
-        cover = torch.zeros(thw, dtype=torch.int32)
-        for (t0, t1, h0, h1, w0, w1) in boxes:
-            cover[t0:t1, h0:h1, w0:w1] += 1
-        assert (cover == 1).all()
-
-
-@pytest.mark.parametrize("variant", ["3b", "7b"])
-def test_layout_tables(pkg, variant):
-    import importlib
-    dit = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.dit")
-    T, Hp, Wp, l = 3, 20, 36, 58
-    L = T * Hp * Wp
-    for shifted in (False, True):
-        lay, size_rows = dit.build_layout(T, Hp, Wp, l, shifted, variant, "cpu")
-        assert lay.total == L + lay.n_win * l
-        assert lay.cu_seqlens[-1].item() == lay.total and lay.cu_seqlens[0].item() == 0
-        assert sorted(lay.out_row_map.tolist()) == list(range(lay.total))       # a permutation
-        vid_rows = lay.row_src >= 0
-        assert sorted(lay.row_src[vid_rows].tolist()) == list(range(L))
-        assert torch.equal(lay.out_row_map[vid_rows], lay.row_src[vid_rows])
-        tgt, lens, loc = dit_oracle.window_token_index(T, Hp, Wp, dit.window_boxes(T, Hp, Wp, shifted))
-        assert torch.equal(lay.row_src[vid_rows].long(), tgt)
-        if variant == "3b":
-            assert torch.equal(lay.row_rope[vid_rows].long(), loc[:, :3] + torch.tensor([l, 0, 0]))
-        fr = torch.linspace(1, 10, 10) if variant == "7b" else torch.arange(1, 22).float()
-        c, s = dit.rope_tables(fr, variant, int(lay.row_rope.max()) + 1, size_rows)
-        assert c.shape == s.shape and c.shape[0] > int(lay.row_rope.max())
-
-
-def test_rope_tables_match_oracle(pkg):
-    import importlib
-    dit = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.dit")
-    T, Hp, Wp, l = 3, 20, 36, 58
-    boxes = dit.window_boxes(T, Hp, Wp, True)
-    _, _, loc = dit_oracle.window_token_index(T, Hp, Wp, boxes)
-    for variant, freqs in (("3b", (1.0 / (10000 ** (torch.arange(0, 42, 2).float() / 42))).half()),
-                           ("7b", (torch.linspace(1.0, 128.0, 10) * torch.pi).half())):
-        lay, size_rows = dit.build_layout(T, Hp, Wp, l, True, variant, "cpu")
-        c, s = dit.rope_tables(freqs, variant, int(lay.row_rope.max()) + 1, size_rows)
-        vid_rows = lay.row_src >= 0
-        rr = lay.row_rope[vid_rows].long()
-        got = torch.cat([c[rr[:, a]].repeat_interleave(2, -1) for a in range(3)], -1)
-        if variant == "3b":
-            (cv, sv), _ = dit_oracle.rope_cos_sin_3b(freqs, loc, l)
-        else:
-            cv, sv = dit_oracle.rope_cos_sin_7b(freqs, loc)
-        assert torch.equal(got, cv)
 
 
 def test_padding_and_partition(pkg):

@@ -289,8 +289,8 @@ def test_dit_native_runtime_equals_python_sequencing(pkg, name):
     out_n = eng(vid.cuda(), txt.cuda(), [[T, H, W]], [[l]]).vid_sample.clone()
     eng.native = False
     out_p = eng(vid.cuda(), txt.cuda(), [[T, H, W]], [[l]]).vid_sample
-    # same kernels, same order, same tables (the RoPE tables come from libm in C++ and from torch here: identical except
-    # at fp16 rounding ties, tests/test_native_geometry_cpu.py) -> bit-identical output
+    # same kernels, same order, same tables (the Python sequencing reads the handle's, svr2_dit_geometry) -> bit-identical
+    # output
     assert torch.equal(out_n, out_p), f"{name}: native vs python sequencing {psnr(out_n, out_p):.1f} dB"
     assert eng.workspace_bytes(T, H, W, l) > 0
     eng.native = True

@@ -1,5 +1,6 @@
 """-m gpu: every C-ABI op of libsvr2.so against a plain torch fp32 restatement of the same
 reference op (floating point kernels; tolerances are stated per test)."""
+import contextlib
 import math
 
 import pytest
@@ -273,14 +274,30 @@ def test_qk_norm_rope_window(svr2lib):
     assert torch.equal(v.float(), rows[:, 2])
 
 
+@contextlib.contextmanager
+def geometry_handle(svr2lib, variant, heads, freqs, layers=4):
+    """A DiT handle that holds nothing but every layer's RoPE frequencies: enough for svr2_dit_geometry."""
+    desc = svr2lib.ModelDesc(variant=0 if variant == "3b" else 1, dim=heads * 128, heads=heads, layers=layers,
+                             mm_layers=layers, txt_in_dim=64, in_ch=33, out_ch=16, mlp_kind=0, mlp_hidden=256, out_norm=1,
+                             last_vid_only=0, eps=1e-5, timestep=1000.0)
+    h = svr2lib.engine_create(desc, torch.cuda.current_device())
+    try:
+        svr2lib.engine_load(h, {f"{i}.rope_freqs": freqs for i in range(layers)}, copy=True)
+        yield h
+    finally:
+        svr2lib.engine_destroy(h)
+
+
 @pytest.mark.parametrize("variant,heads,geom", [("3b", 2, (3, 20, 36)), ("3b", 4, (5, 34, 60)), ("7b", 2, (2, 20, 36)),
-                                                ("3b", 20, (1, 10, 14))])
-def test_linear_qkv_rope_fused_vs_unfused(pkg, svr2lib, variant, heads, geom):
+                                                ("3b", 20, (1, 10, 14)),
+                                                # full width at the latents of a 4K shard and a 17-frame 1080p clip
+                                                ("3b", 20, (2, 135, 240)), ("7b", 24, (2, 135, 240)),
+                                                ("3b", 20, (5, 68, 120)), ("7b", 24, (5, 68, 120))])
+def test_linear_qkv_rope_fused_vs_unfused(svr2lib, variant, heads, geom):
     """QKV GEMM with q/k RMSNorm + RoPE + window scatter in its epilogue (svr2_linear_qkv_rope_bf16) + the row-subset
     kernel for the text rows, against the two-kernel path (svr2_linear_bf16 -> svr2_qk_norm_rope_window_bf16) on the real
-    window layouts (regular and shifted): v bit-equal, q/k equal up to the summation order of the per-head RMS."""
-    import importlib
-    dit = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.dit")
+    window layouts (regular and shifted, svr2_dit_geometry): v bit-equal, q/k equal up to the summation order of the
+    per-head RMS."""
     T, Hp, Wp = geom
     l, d, inner = 58, heads * 128, heads * 128
     L = T * Hp * Wp
@@ -292,28 +309,62 @@ def test_linear_qkv_rope_fused_vs_unfused(pkg, svr2lib, variant, heads, geom):
         freqs = (1.0 / (10000 ** (torch.arange(0, 42, 2)[:21].float() / 42))).half()
     else:
         freqs = (torch.linspace(1.0, 128.0, 10) * math.pi).half()
-    for shifted in (False, True):
-        lay, size_rows = dit.build_layout(T, Hp, Wp, l, shifted, variant, DEV)
-        c, s = dit.rope_tables(freqs, variant, int(lay.row_rope.max().item()) + 1, size_rows)
-        cos_t, sin_t = c.to(DEV), s.to(DEV)
-        nf = cos_t.shape[1]
-        P = svr2lib.ptr
-        qkv_v, qkv_t = svr2lib.linear(a_v, w_v), svr2lib.linear(a_t, w_t)
-        ref = [torch.zeros(lay.total, heads, 128, device=DEV, dtype=torch.bfloat16) for _ in range(3)]
-        svr2lib.call("svr2_qk_norm_rope_window_bf16", P(qkv_v), P(qkv_t), P(lay.row_src), P(lay.row_rope), P(cos_t),
-                     P(sin_t), nf, P(nq_v), P(nk_v), P(nq_t), P(nk_t), 1e-5, lay.total, heads, *(P(t) for t in ref),
-                     svr2lib.stream())
-        got = [torch.zeros_like(t) for t in ref]
-        svr2lib.call("svr2_linear_qkv_rope_bf16", P(a_v), d, P(w_v), d, L, heads, d, P(lay.tok_dst), P(lay.tok_rope),
-                     P(cos_t), P(sin_t), nf, P(nqk), 1e-5, *(P(t) for t in got), svr2lib.stream())
-        svr2lib.call("svr2_qk_norm_rope_rows_bf16", None, P(qkv_t), P(lay.row_src), P(lay.row_rope), P(cos_t), P(sin_t),
-                     nf, P(nq_v), P(nk_v), P(nq_t), P(nk_t), 1e-5, P(lay.txt_rows), lay.txt_rows.numel(), heads,
-                     *(P(t) for t in got), svr2lib.stream())
-        assert torch.equal(got[2], ref[2]), "v rows must be bit-equal"
-        for name, g_, r_ in (("q", got[0], ref[0]), ("k", got[1], ref[1])):
-            dlt = (g_.float() - r_.float()).abs()
-            assert (dlt == 0).float().mean() > 0.98 and dlt.max() <= 2 ** -6 * r_.abs().max().item(), \
-                f"{name} shifted={shifted}: {(dlt == 0).float().mean():.4f} equal, max {dlt.max():.4f}"
+    P = svr2lib.ptr
+    with geometry_handle(svr2lib, variant, heads, freqs) as h:
+        for layer in (0, 1):
+            shifted = bool(layer)
+            g = svr2lib.dit_geometry(h, T, 2 * Hp, 2 * Wp, l, layer)
+            rope = (g.rope_cos, g.rope_sin, g.nfreq)
+            qkv_v, qkv_t = svr2lib.linear(a_v, w_v), svr2lib.linear(a_t, w_t)
+            ref = [torch.zeros(g.total, heads, 128, device=DEV, dtype=torch.bfloat16) for _ in range(3)]
+            svr2lib.call("svr2_qk_norm_rope_window_bf16", P(qkv_v), P(qkv_t), g.row_src, g.row_rope, *rope, P(nq_v),
+                         P(nk_v), P(nq_t), P(nk_t), 1e-5, g.total, heads, *(P(t) for t in ref), svr2lib.stream())
+            got = [torch.zeros_like(t) for t in ref]
+            svr2lib.call("svr2_linear_qkv_rope_bf16", P(a_v), d, P(w_v), d, L, heads, d, g.tok_dst, g.tok_rope, *rope,
+                         P(nqk), 1e-5, *(P(t) for t in got), svr2lib.stream())
+            svr2lib.call("svr2_qk_norm_rope_rows_bf16", None, P(qkv_t), g.row_src, g.row_rope, *rope, P(nq_v), P(nk_v),
+                         P(nq_t), P(nk_t), 1e-5, g.txt_rows, g.n_txt_rows, heads, *(P(t) for t in got), svr2lib.stream())
+            assert torch.equal(got[2], ref[2]), "v rows must be bit-equal"
+            for name, g_, r_ in (("q", got[0], ref[0]), ("k", got[1], ref[1])):
+                dlt = (g_.float() - r_.float()).abs()
+                assert (dlt == 0).float().mean() > 0.98 and dlt.max() <= 2 ** -6 * r_.abs().max().item(), \
+                    f"{name} shifted={shifted}: {(dlt == 0).float().mean():.4f} equal, max {dlt.max():.4f}"
+
+
+@pytest.mark.parametrize("variant", ["3b", "7b"])
+def test_dit_geometry_entry_point(svr2lib, variant):
+    """svr2_dit_geometry: the handle's device tables equal the oracle (as in tests/test_native_geometry_cpu.py); even
+    layers use the regular windows, odd layers the shifted ones; fuse_qkv follows the heads and the RoPE width; and it
+    refuses what svr2_dit_forward refuses, a VAE handle and a layer outside [0, layers)."""
+    from test_native_geometry_cpu import check_against_oracle, rope_freqs
+    freqs = rope_freqs(variant, torch.float16)
+    l = 58
+    ints = ("cu_seqlens", "row_src", "row_rope", "out_row_map", "tok_dst", "tok_rope", "txt_rows")
+    with geometry_handle(svr2lib, variant, 2, freqs) as h:
+        for T, Hp, Wp in ((3, 20, 36), (3, 135, 240)):
+            for layer in (0, 1, 2, 3):
+                g = svr2lib.dit_geometry(h, T, 2 * Hp, 2 * Wp, l, layer)
+                L = T * Hp * Wp
+                sizes = dict(cu_seqlens=g.n_win + 1, row_src=g.total, row_rope=3 * g.total, out_row_map=g.total,
+                             tok_dst=L, tok_rope=3 * L, txt_rows=g.n_txt_rows)
+                got = {n: getattr(g, n) for n in ("n_win", "total", "max_len", "n_txt_rows", "nfreq", "rope_rows")}
+                got.update({n: svr2lib.host_copy(getattr(g, n), (sizes[n],), torch.int32) for n in ints})
+                got.update({n: svr2lib.host_copy(getattr(g, n), (g.rope_rows, g.nfreq), torch.float32)
+                            for n in ("rope_cos", "rope_sin")})
+                check_against_oracle(got, variant, T, Hp, Wp, l, bool(layer & 1), freqs)
+                assert g.fuse_qkv == 1
+        for bad in ((3, 41, 72, l, 0), (3, 40, 72, l, 4), (3, 40, 72, l, -1), (3, 40, 72, 0, 0), (0, 40, 72, l, 0)):
+            with pytest.raises(svr2lib.Svr2Error):
+                svr2lib.dit_geometry(h, *bad)
+    for heads, nfreq, fused in ((2, 21, 1), (2, 10, 1), (4, 21, 1), (3, 21, 0), (3, 10, 0), (2, 16, 0)):
+        with geometry_handle(svr2lib, variant, heads, torch.linspace(0.5, 2.0, nfreq).half()) as h:
+            assert svr2lib.dit_geometry(h, 1, 16, 24, l, 0).fuse_qkv == fused, (heads, nfreq)
+    vae = svr2lib.engine_create(svr2lib.ModelDesc(variant=2), torch.cuda.current_device())
+    try:
+        with pytest.raises(svr2lib.Svr2Error, match="VAE"):
+            svr2lib.dit_geometry(vae, 1, 16, 24, l, 0)
+    finally:
+        svr2lib.engine_destroy(vae)
 
 
 @pytest.mark.parametrize("C,hw,frames,silu", [(128, 24 * 36, 3, 1), (256, 1000, 2, 1), (512, 77, 2, 0),
