@@ -127,6 +127,7 @@ struct Run {
   char* base;          // nullptr: dry run (plan only)
   void* stream;
   bool slicing = false, first = true;
+  bool tails = true;                                 // a later slice reads this slice's tails (false: the last decode slice)
   std::unordered_map<std::string, size_t> state;     // layer key -> top-region offset of the previous slice's tail
   int64_t launches = 0;
   int rc = SVR2_OK;
@@ -178,19 +179,20 @@ struct Run {
   bool has(const std::string& name) { return find(e, name) != nullptr; }
 
   // Slice boundary: the halo of a tensor that feeds a causal conv is the previous slice's tail at the same layer
-  // (InflatedCausalConv3d.memory, causal_inflation_lib.py:306-352); remember this slice's tail.
+  // (InflatedCausalConv3d.memory, causal_inflation_lib.py:306-352); remember this slice's tail unless no later slice
+  // runs (the last decode slice).
   void halo(const Act& y, const std::string& key) {
     if (!slicing || y.pad == 0 || !ok()) return;
     const size_t bytes = (size_t)y.pad * y.frame_bytes();
     auto it = state.find(key);
-    if (it == state.end()) {
+    if (it != state.end()) {
+      if (!dry() && !dev_copy(P(y.off), P(it->second), bytes, stream)) err(SVR2_ERR_CUDA, "svr2_vae: halo copy failed");
+    } else if (tails) {
       const size_t off = A.alloc_top(bytes);
       if (off == NONE) { err(SVR2_ERR_ARG, "svr2_vae: workspace smaller than svr2_vae_workspace_bytes()"); return; }
       it = state.emplace(key, off).first;
-    } else if (!dry()) {
-      if (!dev_copy(P(y.off), P(it->second), bytes, stream)) err(SVR2_ERR_CUDA, "svr2_vae: halo copy failed");
     }
-    if (!dry() && ok()) {
+    if (tails && !dry() && ok()) {
       if (!dev_copy(P(it->second), P(y.off) + (size_t)y.T * y.frame_bytes(), bytes, stream))
         err(SVR2_ERR_CUDA, "svr2_vae: halo copy failed");
     }
@@ -411,8 +413,10 @@ struct Run {
     return resnet(b, p + "resnets.1.", 0);
   }
 
-  // Upsample3D.forward (attn_video_vae.py:110-174); consumes x
-  Act upsample(Act& x, const std::string& p, bool temporal) {
+  // Upsample3D.forward (attn_video_vae.py:110-174); consumes x.  keep > 0: only the first `keep` shuffled frames are
+  // wanted — every layer after the decoder's last temporal upsampler is causal frame by frame, so the conv and
+  // everything after it run on those frames alone (the block keeps its full size: it is released whole)
+  Act upsample(Act& x, const std::string& p, bool temporal, int keep = 0) {
     const Tensor *w = weight(p + "upscale_conv.weight"), *b = weight(p + "upscale_conv.bias");
     const int z = temporal ? 2 : 1;
     const int T_out = x.T * z - (temporal && first ? 1 : 0);      // remove_head only drops (f=0, z=1) of the clip's first slice
@@ -421,6 +425,7 @@ struct Run {
       ck(svr2_upsample_shuffle_bf16(P(x.off) + (size_t)x.pad * x.frame_bytes(), x.T, x.H, x.W, x.C, w->ptr, b->ptr, temporal, first,
                                     P(y.off), 2, first, stream));
     drop(x);
+    if (keep > 0 && keep < y.T) y.T = keep;
     halo(y, p + "shuffle");
     Act c = conv(y, p + "conv", 0, nullptr, 1, 1, true);
     drop(y);
@@ -428,8 +433,9 @@ struct Run {
   }
 
   // One temporal slice of Decoder3D.forward: z (16 channels, T frames of h x w, channel stride zin_cs elements) ->
-  // out (3 channels, T' frames of 8h x 8w written at out, channel stride out_cs); T' = 4T-3 for the first slice, else 4T
-  void decode_slice(const void* zin, int dt, int64_t zin_cs, int T, int h, int w, void* out, int64_t out_cs) {
+  // out (3 channels, the first `keep` of the slice's T' frames of 8h x 8w written at out, channel stride out_cs);
+  // T' = 4T-3 for the first slice, else 4T
+  void decode_slice(const void* zin, int dt, int64_t zin_cs, int T, int h, int w, void* out, int64_t out_cs, int keep) {
     Act x = act(T, h, w, 64, 2);
     if (!dry() && ok()) ck(ncdhw_to_ndhwc_strided(zin, dt, 16, T, h, w, zin_cs, P(x.off), 64, 2, 1.0f, stream));
     halo(x, "decoder.in");
@@ -444,11 +450,12 @@ struct Run {
       }
       if (i < 3) {
         snprintf(name, sizeof name, "decoder.up_blocks.%d.upsamplers.0.", i);
-        m = upsample(m, name, i < 2);
+        m = upsample(m, name, i < 2, i == 1 ? keep : 0);
       }
     }
     Act g = gn(m, "decoder.conv_norm_out", true, 2);
     drop(m);
+    if (ok() && g.T != keep) err(SVR2_ERR_ARG, "svr2_vae_decode: decoded frame count differs from the plan");
     // conv_out (128 -> 3): per-tap channel contraction as ONE GEMM over all input pixels (x read once, not 27 times),
     // fp32 z[tap*3+co][pixel], then the 27-tap gather writes NCDHW directly
     const Tensor *wt = weight("decoder.conv_out.weight"), *bo = weight("decoder.conv_out.bias");
@@ -504,19 +511,25 @@ struct Run {
     drop(c);
   }
 
-  // slicing_decode (attn_video_vae.py:1279-1300): the first slice is latent frame 0 plus `size` frames, then `size` each
-  void decode(const void* z, int dt, int T, int h, int w, int size, void* out) {
+  // slicing_decode (attn_video_vae.py:1279-1300): the first slice is latent frame 0 plus `size` frames, then `size` each.
+  // Only the first `frames` (1 .. 4T-3) output frames are computed: the decoder is causal in time, so the reference's
+  // decode-then-crop returns the same values.  Slices past them do not run, the last one that does is trimmed.
+  void decode(const void* z, int dt, int T, int h, int w, int size, int frames, void* out) {
     const int esz = dt == 0 ? 4 : 2;
-    const int64_t zin_cs = (int64_t)T * h * w, out_cs = (int64_t)(4 * T - 3) * 64 * h * w;
+    const int64_t zin_cs = (int64_t)T * h * w, out_cs = (int64_t)frames * 64 * h * w;
     if (size <= 0 || T - 1 <= size) {
-      decode_slice(z, dt, zin_cs, T, h, w, out, out_cs);
+      decode_slice(z, dt, zin_cs, T, h, w, out, out_cs, frames);
       return;
     }
     slicing = true;
     for (int a = 0, b = 1 + size; a < T && ok(); a = b, b = (b + size < T ? b + size : T)) {
       first = a == 0;
-      const int64_t o0 = a == 0 ? 0 : 4 * (int64_t)a - 3;
-      decode_slice((const char*)z + (size_t)a * h * w * esz, dt, zin_cs, b - a, h, w, (char*)out + (size_t)o0 * 64 * h * w * 2, out_cs);
+      const int o0 = a == 0 ? 0 : 4 * a - 3, n_out = 4 * (b - a) - (first ? 3 : 0);
+      const int keep = frames - o0 < n_out ? frames - o0 : n_out;
+      if (keep <= 0) break;                // this and every later slice lie past the wanted frames
+      tails = o0 + n_out < frames;         // a later slice runs and continues from this one's tails
+      decode_slice((const char*)z + (size_t)a * h * w * esz, dt, zin_cs, b - a, h, w, (char*)out + (size_t)o0 * 64 * h * w * 2,
+                   out_cs, keep);
     }
   }
 
@@ -555,17 +568,27 @@ int check_args(svr2_engine* e, const char* what, int T, int H, int W, int mult) 
   return SVR2_OK;
 }
 
-size_t plan_bytes(svr2_engine* e, int encode, int T, int H, int W, int slice_frames) {
+// decode: the number of output frames wanted, 1 .. 4T-3
+int check_frames(svr2_engine* e, const char* what, int T, int frames) {
+  if (frames >= 1 && frames <= 4 * T - 3) return SVR2_OK;
+  char buf[160];
+  snprintf(buf, sizeof buf, "%s: frames = %d, a decode of %d latent frames returns 1 .. %d frames", what, frames, T, 4 * T - 3);
+  return fail(e, SVR2_ERR_ARG, buf);
+}
+
+// frames: output frames of a decode (ignored by an encode)
+size_t plan_bytes(svr2_engine* e, int encode, int T, int H, int W, int slice_frames, int frames) {
   Run r(e, ~(size_t)0 / 2, nullptr, nullptr);
   if (encode) r.encode(nullptr, 1, T, H, W, slice_frames, nullptr);
-  else r.decode(nullptr, 1, T, H, W, slice_frames, nullptr);
+  else r.decode(nullptr, 1, T, H, W, slice_frames, frames, nullptr);
   return r.ok() ? r.A.need() : 0;
 }
 
-int run(svr2_engine* e, int encode, const void* in, int dt, int T, int H, int W, int slice_frames, void* out, void* ws,
-        size_t ws_bytes, void* stream) {
+int run(svr2_engine* e, int encode, const void* in, int dt, int T, int H, int W, int slice_frames, int frames, void* out,
+        void* ws, size_t ws_bytes, void* stream) {
   const char* what = encode ? "svr2_vae_encode" : "svr2_vae_decode";
   int rc = check_args(e, what, T, H, W, encode ? 8 : 1);
+  if (!rc && !encode) rc = check_frames(e, what, T, frames);
   if (rc) return rc;
   if (!in || !out) return fail(e, SVR2_ERR_ARG, "svr2_vae: null input / output");
   if (dt < 0 || dt > 2) return fail(e, SVR2_ERR_ARG, "svr2_vae: dtype must be 0 (f32), 1 (bf16) or 2 (f16)");
@@ -574,7 +597,7 @@ int run(svr2_engine* e, int encode, const void* in, int dt, int T, int H, int W,
   cudaGetDevice(&cur);
   if (cur != e->device) return fail(e, SVR2_ERR_ARG, "svr2_vae: the handle's device is not the current device");
 #endif
-  const size_t need = plan_bytes(e, encode, T, H, W, slice_frames);
+  const size_t need = plan_bytes(e, encode, T, H, W, slice_frames, frames);
   if (!need) return SVR2_ERR_ARG;      // message already recorded
   if (!e->vae) e->vae = new VaeState();
   char* base;
@@ -599,7 +622,7 @@ int run(svr2_engine* e, int encode, const void* in, int dt, int T, int H, int W,
   }
   Run r(e, need, base, stream);
   if (encode) r.encode(in, dt, T, H, W, slice_frames, out);
-  else r.decode(in, dt, T, H, W, slice_frames, out);
+  else r.decode(in, dt, T, H, W, slice_frames, frames, out);
   e->vae->last_launches = r.launches;
   return r.rc;
 }
@@ -613,17 +636,29 @@ using namespace svr2;
 // H x W latent pixels) uses with temporal slices of `slice_frames` (0 = un-sliced).  Exact: the dry run of the same code.
 extern "C" size_t svr2_vae_workspace_bytes(svr2_t* e, int direction, int T, int H, int W, int slice_frames) {
   if (check_args(e, "svr2_vae_workspace_bytes", T, H, W, direction == 0 ? 8 : 1)) return 0;
-  return plan_bytes(e, direction == 0, T, H, W, slice_frames);
+  return plan_bytes(e, direction == 0, T, H, W, slice_frames, 4 * T - 3);
+}
+
+// Bytes of workspace one decode of T latent frames that returns only the first `frames` output frames uses.  Exact.
+extern "C" size_t svr2_vae_decode_frames_workspace_bytes(svr2_t* e, int T, int h, int w, int slice_frames, int frames) {
+  const char* what = "svr2_vae_decode_frames_workspace_bytes";
+  if (check_args(e, what, T, h, w, 1) || check_frames(e, what, T, frames)) return 0;
+  return plan_bytes(e, 0, T, h, w, slice_frames, frames);
 }
 
 extern "C" int svr2_vae_encode(svr2_t* e, const void* x, int x_dtype, int T, int H, int W, int slice_frames, void* latent,
                                void* workspace, size_t workspace_bytes, void* stream) {
-  return run(e, 1, x, x_dtype, T, H, W, slice_frames, latent, workspace, workspace_bytes, stream);
+  return run(e, 1, x, x_dtype, T, H, W, slice_frames, 0, latent, workspace, workspace_bytes, stream);
 }
 
 extern "C" int svr2_vae_decode(svr2_t* e, const void* z, int z_dtype, int T, int h, int w, int slice_frames, void* sample,
                                void* workspace, size_t workspace_bytes, void* stream) {
-  return run(e, 0, z, z_dtype, T, h, w, slice_frames, sample, workspace, workspace_bytes, stream);
+  return run(e, 0, z, z_dtype, T, h, w, slice_frames, 4 * T - 3, sample, workspace, workspace_bytes, stream);
+}
+
+extern "C" int svr2_vae_decode_frames(svr2_t* e, const void* z, int z_dtype, int T, int h, int w, int slice_frames, int frames,
+                                      void* sample, void* workspace, size_t workspace_bytes, void* stream) {
+  return run(e, 0, z, z_dtype, T, h, w, slice_frames, frames, sample, workspace, workspace_bytes, stream);
 }
 
 // kernels launched by the last svr2_vae_encode / svr2_vae_decode of this handle (bench.py's gpu_launches)

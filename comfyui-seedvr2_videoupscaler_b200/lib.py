@@ -51,6 +51,8 @@ SIGNATURES = {
     "svr2_vae_workspace_bytes": [_P, c_int, c_int, c_int, c_int, c_int],
     "svr2_vae_encode": [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
     "svr2_vae_decode": [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
+    "svr2_vae_decode_frames_workspace_bytes": [_P, c_int, c_int, c_int, c_int, c_int],
+    "svr2_vae_decode_frames": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
     "svr2_vae_last_launches": [_P],
     "svr2_linear_bf16": [_P, c_int64, _P, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int64, c_float, _P],
     "svr2_conv3d_bf16": [_P, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -17,6 +17,7 @@ device memory independent of the length.
 """
 from __future__ import annotations
 
+import inspect
 from typing import Dict, Iterator, Optional, Tuple
 
 import torch
@@ -53,6 +54,15 @@ def pad_video_temporal(frames: torch.Tensor, count: int = 0, prepend: bool = Fal
         return torch.cat([repeated, rev, frames] if prepend else [frames, rev, repeated], 0)
     rev = frames[1:count + 1].flip(0) if prepend else frames[-count - 1:-1].flip(0)
     return torch.cat([rev, frames] if prepend else [frames, rev], 0)
+
+
+def _frames_kw(phase, frames: int) -> dict:
+    """``{"frames": frames}`` for a phase method (``vae_decode``, ``clip_workspace``) that takes the decoded frame count;
+    ``{}`` for a replacement with the plain signature, which then decodes (plans) every frame and the caller crops."""
+    try:
+        return {"frames": frames} if "frames" in inspect.signature(phase).parameters else {}
+    except (TypeError, ValueError):
+        return {}
 
 
 class SeedVR2Engine:
@@ -92,24 +102,27 @@ class SeedVR2Engine:
 
     # ---- VideoDiffusionInfer.vae_decode -----------------------------------
     @torch.no_grad()
-    def vae_decode(self, latent: torch.Tensor, workspace=None) -> torch.Tensor:
-        """latent (T',h,w,16) -> sample (3,T,H,W) bf16 in ~[-1,1]."""
+    def vae_decode(self, latent: torch.Tensor, workspace=None, frames: Optional[int] = None) -> torch.Tensor:
+        """latent (T',h,w,16) -> sample (3,T,H,W) bf16 in ~[-1,1]; ``frames``: only the first ``frames`` of the T = 4T'-3
+        frames are decoded (the same values; None: all)."""
         z = latent.permute(3, 0, 1, 2)[None]
         z = z / SCALING_FACTOR + SHIFTING_FACTOR
-        return self.vae.decode(z, workspace=workspace).sample[0]
+        return self.vae.decode(z, workspace=workspace, frames=frames).sample[0]
 
-    def clip_workspace(self, T: int, Hp: int, Wp: int) -> Optional[torch.Tensor]:
-        """ONE workspace for the three phases of a clip of T (4n+1) frames at Hp x Wp (multiples of 16): the maximum of
-        the exact needs of VAE encode, the DiT forward and VAE decode (svr2_vae_workspace_bytes / svr2_workspace_bytes),
-        with the VAE passes temporally sliced until they fit the free HBM.  The phases run one after the other on one
-        stream, so they can share the bytes; the block is the engine's resident workspace (lib.workspace: kept between clips,
-        grown on demand; the capture pool inside a CUDA graph).  None when a phase runs on the Python sequencing (profiling)."""
+    def clip_workspace(self, T: int, Hp: int, Wp: int, frames: Optional[int] = None) -> Optional[torch.Tensor]:
+        """ONE workspace for the three phases of a clip of T (4n+1) frames at Hp x Wp (multiples of 16) of which the first
+        ``frames`` are decoded (None: all): the maximum of the exact needs of VAE encode, the DiT forward and VAE decode
+        (svr2_vae_workspace_bytes / svr2_workspace_bytes / svr2_vae_decode_frames_workspace_bytes), with the VAE passes
+        temporally sliced until they fit the free HBM.  The phases run one after the other on one stream, so they can
+        share the bytes; the block is the engine's resident workspace (lib.workspace: kept between clips, grown on demand;
+        the capture pool inside a CUDA graph).  None when a phase runs on the Python sequencing (profiling)."""
         from . import lib
         if not (self.vae._use_native() and self.dit.native and lib.PROFILER is None):
             return None
         Tl, h, w = (T - 1) // 4 + 1, Hp // 8, Wp // 8
         budget = int(0.92 * self.vae._free_bytes()) - 2 * 3 * T * Hp * Wp * 2      # the decoded clip and its crop
-        need = max(self.vae.plan_slices(True, T, Hp, Wp, budget)[1], self.vae.plan_slices(False, Tl, h, w, budget)[1],
+        need = max(self.vae.plan_slices(True, T, Hp, Wp, budget)[1],
+                   self.vae.plan_slices(False, Tl, h, w, budget, frames=frames)[1],
                    self.dit.workspace_bytes(Tl, h, w, self.txt.shape[0]))
         return lib.workspace(need, self.device)
 
@@ -208,7 +221,8 @@ class SeedVR2Engine:
         tf = preprocess.VideoTransform(res, max_resolution)
         H0, W0 = tf.true_size(frames.shape[1], frames.shape[2])
         x = tf.run(x, channels_last=True)                           # (3, T, Hp, Wp) bf16 in [-1,1]
-        ws = self.clip_workspace(x.shape[1], x.shape[2], x.shape[3])
+        # only the T0 real frames are decoded: the padding frames' decoder work after its last temporal upsampler is skipped
+        ws = self.clip_workspace(x.shape[1], x.shape[2], x.shape[3], **_frames_kw(self.clip_workspace, T0))
         kw = {} if ws is None else {"workspace": ws}
         x_enc = x
         if input_noise_scale > 0:
@@ -226,7 +240,7 @@ class SeedVR2Engine:
                 latent_noise = gen_noise.draw_latent_noise(latent.shape, g, self.device)
         aug = dict(latent_noise=latent_noise, latent_noise_scale=latent_noise_scale) if latent_noise_scale > 0 else {}
         x0 = self.inference(noise, latent, **kw, **aug)
-        y = self.vae_decode(x0, **kw)                               # (3,T,H,W)
+        y = self.vae_decode(x0, **kw, **_frames_kw(self.vae_decode, T0))      # (3,T0,H,W), or (3,T,H,W)
         del ws, kw
         sample = y[:, :T0, :H0, :W0].permute(1, 0, 2, 3)            # t c h w, the layout of phase 4
         style = x[:, :T0, :H0, :W0].permute(1, 0, 2, 3)            # the transformed input clip in [-1,1]

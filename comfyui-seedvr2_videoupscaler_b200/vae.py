@@ -119,15 +119,19 @@ class B200VideoVAE(EngineModule):
             tensors[k] = t
         return tensors
 
-    def workspace_bytes(self, encode: bool, T: int, H: int, W: int, slice_frames: int = 0) -> int:
+    def workspace_bytes(self, encode: bool, T: int, H: int, W: int, slice_frames: int = 0,
+                        frames: Optional[int] = None) -> int:
         """Exact workspace of one native encode (T sample frames of H x W) / decode (T latent frames of H x W latent
-        pixels) with temporal slices of ``slice_frames`` (0 = un-sliced)."""
-        key = (bool(encode), T, H, W, slice_frames)
+        pixels) with temporal slices of ``slice_frames`` (0 = un-sliced); ``frames``: the decoded frames wanted (None:
+        all 4T-3)."""
+        frames = None if encode else (4 * T - 3 if frames is None else frames)
+        key = (bool(encode), T, H, W, slice_frames, frames)
         if key not in self._ws_bytes:
-            n = int(lib.load().svr2_vae_workspace_bytes(self.native_handle(), 0 if encode else 1, T, H, W, slice_frames))
+            L, h = lib.load(), self.native_handle()
+            n = int(L.svr2_vae_workspace_bytes(h, 0, T, H, W, slice_frames) if encode
+                    else L.svr2_vae_decode_frames_workspace_bytes(h, T, H, W, slice_frames, frames))
             if n <= 0:
-                raise lib.Svr2Error("svr2_vae_workspace_bytes failed: "
-                                    + lib.load().svr2_engine_last_error(self.native_handle()).decode())
+                raise lib.Svr2Error("svr2_vae workspace query failed: " + L.svr2_engine_last_error(h).decode())
             self._ws_bytes[key] = n
         return self._ws_bytes[key]
 
@@ -140,15 +144,18 @@ class B200VideoVAE(EngineModule):
         held = 0 if torch.cuda.is_current_stream_capturing() else lib.workspace_held(self.device)
         return free + torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device) + held
 
-    def plan_slices(self, encode: bool, T: int, H: int, W: int, budget: Optional[int] = None):
+    def plan_slices(self, encode: bool, T: int, H: int, W: int, budget: Optional[int] = None,
+                    frames: Optional[int] = None):
         """(slice_frames, workspace bytes) of a native encode (T sample frames of H x W) / decode (T latent frames of
-        H x W latent pixels): the longest temporal slice — un-sliced first, then set_causal_slicing's split, then shorter
-        ones — whose EXACT workspace fits ``budget`` bytes (default: 92 % of the free HBM incl. torch's cached blocks)."""
+        H x W latent pixels; ``frames``: the decoded frames wanted, None: all): the longest temporal slice — un-sliced
+        first, then set_causal_slicing's split, then shorter ones — whose EXACT workspace fits ``budget`` bytes (default:
+        92 % of the free HBM incl. torch's cached blocks)."""
         step = 4 if encode else 1
         cap = None if self.split_size is None else (max(4, self.split_size // 4 * 4) if encode else max(1, self.split_size // 4))
         can_slice = not (encode and (T - 1) % 4)       # only 4n+1-frame clips continue the temporal stride phase
         sz = 0 if (cap is None or T - 1 <= cap or not can_slice) else cap
-        need = self.workspace_bytes(encode, T, H, W, sz)
+        fr = {} if frames is None else {"frames": frames}
+        need = self.workspace_bytes(encode, T, H, W, sz, **fr)
         if can_slice:
             if budget is None:
                 budget = int(0.92 * self._free_bytes())
@@ -157,23 +164,29 @@ class B200VideoVAE(EngineModule):
                 if cur <= step:
                     break
                 sz = cur - step
-                need = self.workspace_bytes(encode, T, H, W, sz)
+                need = self.workspace_bytes(encode, T, H, W, sz, **fr)
         return sz, need
 
-    def _native_run(self, encode: bool, src: torch.Tensor, T: int, H: int, W: int, out: torch.Tensor, workspace=None):
+    def _native_run(self, encode: bool, src: torch.Tensor, T: int, H: int, W: int, out: torch.Tensor, workspace=None,
+                    frames: Optional[int] = None):
         """``workspace``: a uint8 CUDA tensor shared by the phases of a clip (pipeline.SeedVR2Engine.clip_workspace) or None —
-        then the engine's resident block (lib.workspace; the capture pool inside a CUDA graph)."""
+        then the engine's resident block (lib.workspace; the capture pool inside a CUDA graph).  ``frames``: decode only
+        the first ``frames`` output frames (None: all)."""
         if workspace is not None:
-            sz, need = self.plan_slices(encode, T, H, W, budget=workspace.numel())
+            sz, need = self.plan_slices(encode, T, H, W, budget=workspace.numel(), frames=frames)
             if need > workspace.numel():
                 raise lib.Svr2Error(f"B200VideoVAE: workspace of {workspace.numel()} bytes given, {need} needed")
             ws = workspace
         else:
-            sz, need = self.plan_slices(encode, T, H, W)
+            sz, need = self.plan_slices(encode, T, H, W, frames=frames)
             ws = lib.workspace(need, self.device)
         dt = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}[src.dtype]
-        lib.call("svr2_vae_encode" if encode else "svr2_vae_decode", self.native_handle(), lib.ptr(src), dt, T, H, W, sz,
-                 lib.ptr(out), lib.ptr(ws), ws.numel(), lib.stream())
+        if encode:
+            lib.call("svr2_vae_encode", self.native_handle(), lib.ptr(src), dt, T, H, W, sz, lib.ptr(out), lib.ptr(ws),
+                     ws.numel(), lib.stream())
+        else:
+            lib.call("svr2_vae_decode_frames", self.native_handle(), lib.ptr(src), dt, T, H, W, sz,
+                     4 * T - 3 if frames is None else frames, lib.ptr(out), lib.ptr(ws), ws.numel(), lib.stream())
         lib.LAUNCHES += int(lib.load().svr2_vae_last_launches(self.native_handle())) - 1
         return out
 
@@ -422,8 +435,10 @@ class B200VideoVAE(EngineModule):
         x = self._attention(x, p + "attentions.0.")
         return self._resnet(x, p + "resnets.1.")
 
-    def _upsample(self, x: Act, p: str, temporal: bool) -> Act:
-        """Upsample3D.forward (attn_video_vae.py:110-174)."""
+    def _upsample(self, x: Act, p: str, temporal: bool, keep: Optional[int] = None) -> Act:
+        """Upsample3D.forward (attn_video_vae.py:110-174).  ``keep``: only the first ``keep`` shuffled frames are wanted
+        (the decoder's last temporal upsampler; every later layer is causal frame by frame): the conv and everything
+        after it run on those frames alone."""
         z = 2 if temporal else 1
         first = self._first                       # remove_head only drops (f=0, z=1) of the clip's first slice
         T_out = x.T * z - (1 if temporal and first else 0)
@@ -432,6 +447,8 @@ class B200VideoVAE(EngineModule):
                  lib.ptr(self.W[p + "upscale_conv.weight"]), lib.ptr(self.W[p + "upscale_conv.bias"]), int(temporal),
                  int(first), lib.ptr(y.buf), 2, int(first), lib.stream(),
                  flops=2.0 * x.T * x.H * x.W * x.C * 4 * z * x.C)
+        if keep is not None and keep < y.T:
+            y = Act(keep, y.H, y.W, y.C, y.pad, self.device, buf=y.buf[:y.pad + keep])
         self._halo(y, p + "shuffle")
         return self._conv(y, p + "conv", stats=True)
 
@@ -461,9 +478,26 @@ class B200VideoVAE(EngineModule):
             cuts.append((cuts[-1][1], min(T, cuts[-1][1] + size)))
         return cuts
 
-    def _run_sliced(self, fn, src: torch.Tensor, cuts):
+    @staticmethod
+    def _decoded_per_slice(cuts, frames: int):
+        """Output frames each decode slice of ``cuts`` computes when only the first ``frames`` are wanted (slice_decode
+        of the native runtime): slices past them are dropped, the last one that runs is trimmed."""
+        keep, o0 = [], 0
+        for a, b in cuts:
+            n_out = 4 * (b - a) - (3 if a == 0 else 0)
+            if frames <= o0:
+                break
+            keep.append(min(frames - o0, n_out))
+            o0 += n_out
+        return keep
+
+    def _run_sliced(self, fn, src: torch.Tensor, cuts, keep=None):
+        """``keep`` (decode): per slice, the output frames ``fn(slice, keep[i])`` computes; slices without an entry do not
+        run.  None: ``fn(slice)`` for every slice."""
+        extra = [()] * len(cuts) if keep is None else [(k,) for k in keep]
         if len(cuts) == 1:
-            return fn(src)
+            return fn(src, *extra[0])
+        cuts = cuts[:len(extra)]
         outs = []
         key = (fn.__name__, tuple(src.shape), tuple(cuts))
         if not torch.cuda.is_current_stream_capturing():
@@ -480,8 +514,8 @@ class B200VideoVAE(EngineModule):
             self._sliced_plans.add(key)
         self._chunk = {"first": True, "state": {}}
         try:
-            for a, b in cuts:
-                outs.append(fn(src[:, a:b].contiguous()))
+            for (a, b), args in zip(cuts, extra):
+                outs.append(fn(src[:, a:b].contiguous(), *args))
                 self._chunk["first"] = False
         finally:
             self._chunk = None
@@ -489,21 +523,30 @@ class B200VideoVAE(EngineModule):
 
     # ---- public API --------------------------------------------------------
     @torch.no_grad()
-    def decode(self, z: torch.Tensor, return_dict=True, tiled=False, tile_size=None, tile_overlap=None, workspace=None):
-        """z (1,16,T,h,w) or (1,16,h,w) -> .sample (1,3,4T-3,8h,8w) bf16 (Decoder3D.forward)."""
+    def decode(self, z: torch.Tensor, return_dict=True, tiled=False, tile_size=None, tile_overlap=None, workspace=None,
+               frames: Optional[int] = None):
+        """z (1,16,T,h,w) or (1,16,h,w) -> .sample (1,3,4T-3,8h,8w) bf16 (Decoder3D.forward).  ``frames``: return only
+        the first ``frames`` (1 .. 4T-3) output frames, the same values; the decoder is causal in time, so the layers
+        after the last temporal upsampler run on those frames alone (the spatially tiled decode decodes all and crops)."""
         self._require_cuda("B200VideoVAE.decode")
         squeeze = z.ndim == 4
         if squeeze:
             z = z.unsqueeze(2)
+        T = z.shape[2]
+        if frames is not None and not 1 <= frames <= 4 * T - 3:
+            raise ValueError(f"frames = {frames}: a decode of {T} latent frames returns 1 .. {4 * T - 3} frames")
         if tiled:
             out = self._tiled(z, False, tile_size or (512, 512), tile_overlap or (64, 64))
+            if frames is not None:
+                out = out[:, :, :frames]
             return VAEOutput(sample=out.squeeze(2) if squeeze else out)
         assert z.shape[0] == 1 and z.shape[1] == 16
         _, _, T, h, w = z.shape
+        F = 4 * T - 3 if frames is None else frames
         zin = z[0].to(self.device)
         if self._use_native():
-            out = torch.empty(1, 3, 4 * T - 3, 8 * h, 8 * w, device=self.device, dtype=torch.bfloat16)
-            self._native_run(False, zin.contiguous(), T, h, w, out, workspace)
+            out = torch.empty(1, 3, F, 8 * h, 8 * w, device=self.device, dtype=torch.bfloat16)
+            self._native_run(False, zin.contiguous(), T, h, w, out, workspace, frames=F)
             return VAEOutput(sample=out.squeeze(2) if squeeze else out)
         if 4 * T - 3 <= self._frames_that_fit(8 * h, 8 * w):         # the whole clip fits: no slicing state needed
             size = T
@@ -511,13 +554,15 @@ class B200VideoVAE(EngineModule):
             size = max(1, self._frames_that_fit(8 * h, 8 * w, self.DEC_STATE_BYTES_PER_PIXEL) // 4)   # latent frames
         if self.split_size is not None:
             size = min(size, max(1, self.split_size // 4))
-        out = self._run_sliced(self._decode_slice, zin, self._plan(T, size))
+        cuts = self._plan(T, size)
+        out = self._run_sliced(self._decode_slice, zin, cuts, self._decoded_per_slice(cuts, F))
         if squeeze:
             out = out.squeeze(2)
         return VAEOutput(sample=out)
 
-    def _decode_slice(self, zin: torch.Tensor) -> torch.Tensor:
-        """One temporal slice: zin (16,T,h,w) -> (1,3,T',8h,8w), T' = 4T-3 for the clip's first slice else 4T."""
+    def _decode_slice(self, zin: torch.Tensor, keep: int) -> torch.Tensor:
+        """One temporal slice: zin (16,T,h,w) -> (1,3,keep,8h,8w), the first ``keep`` of its T' output frames (T' = 4T-3
+        for the clip's first slice else 4T)."""
         dev = self.device
         zin = zin.contiguous()
         _, T, h, w = zin.shape
@@ -531,7 +576,8 @@ class B200VideoVAE(EngineModule):
             for j in range(3):
                 x = self._resnet(x, f"decoder.up_blocks.{i}.resnets.{j}.")
             if i < 3:
-                x = self._upsample(x, f"decoder.up_blocks.{i}.upsamplers.0.", temporal=i < 2)
+                x = self._upsample(x, f"decoder.up_blocks.{i}.upsamplers.0.", temporal=i < 2, keep=keep if i == 1 else None)
+        assert x.T == keep
         x = self._gn(x, "decoder.conv_norm_out", True, 2)
         # conv_out (128 -> 3): per-tap channel contraction as ONE GEMM over all input pixels (x read once, not
         # 27 times), fp32 z[tap*3+co][pixel], then the 27-tap spatial/temporal gather writes NCDHW directly.

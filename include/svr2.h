@@ -142,6 +142,13 @@ int svr2_vae_encode(svr2_t* engine, const void* x, int x_dtype, int T, int H, in
                     void* workspace, size_t workspace_bytes, void* stream);
 int svr2_vae_decode(svr2_t* engine, const void* z, int z_dtype, int T, int h, int w, int slice_frames, void* sample,
                     void* workspace, size_t workspace_bytes, void* stream);
+/* Decode that returns only the first `frames` (1 .. 4T-3) output frames: sample [3, frames, 8h, 8w] bf16, bit-identical to
+ * those frames of svr2_vae_decode (the decoder is causal in time).  After the last temporal upsampler the layers run on the
+ * wanted frames only, and temporal slices past them are not run.  svr2_vae_decode is the frames = 4T-3 case; the
+ * workspace query is exact for the trimmed decode.  frames outside 1 .. 4T-3 is refused (0 bytes / SVR2_ERR_ARG). */
+size_t svr2_vae_decode_frames_workspace_bytes(svr2_t* engine, int T, int h, int w, int slice_frames, int frames);
+int svr2_vae_decode_frames(svr2_t* engine, const void* z, int z_dtype, int T, int h, int w, int slice_frames, int frames,
+                           void* sample, void* workspace, size_t workspace_bytes, void* stream);
 /* kernels launched by the handle's last svr2_vae_encode / svr2_vae_decode */
 int64_t svr2_vae_last_launches(svr2_t* engine);
 
