@@ -63,6 +63,9 @@ struct GemmParams {
   long long out_frame_stride;  // conv/shuffle: elements per output frame
   int out_t_pad;         // leading halo frames in the output tensor (0 or 2)
   int out_dup_head;      // also write frame 0 into the halo frames
+  // ---- conv head fold (SVR2_EPI_FOLD_HEAD): output frames t_o < fold_t read a halo that replicates input frame 0 and
+  // run t_o + 1 temporal taps with the folded weights in B rows [fold_n, fold_n + Cout)
+  int fold_t, fold_n;
   int shuf_c, shuf_z;    // pixel shuffle: channels per output voxel, temporal factor
   int shuf_H, shuf_W;    // input H,W of the shuffle GEMM (rows are (f,h,w))
   int shuf_drop;         // drop the duplicated first output frame (first chunk)
@@ -169,6 +172,14 @@ __device__ __forceinline__ void conv_tile(const GemmParams& p, int m_blk, int& t
   const int trow = rr / p.tiles_w;
   th = band * p.band_h + trow;
   tw = rr - trow * p.tiles_w;
+}
+
+// k-blocks of a conv m-tile: with folded head taps, output frame 0 runs one temporal tap and frame 1 two
+__device__ __forceinline__ int conv_k_blocks(const GemmParams& p, int m_blk) {
+  if (p.fold_t == 0) return p.num_k_blocks;
+  int t_o, th, tw;
+  conv_tile(p, m_blk, t_o, th, tw);
+  return t_o < p.fold_t ? p.num_k_blocks - (p.taps_t - 1 - t_o) * p.taps_h * p.taps_w * p.cin_blocks : p.num_k_blocks;
 }
 
 // L2-aware tile raster: the n-tiles are processed in groups of `g` columns of tiles; inside a group the order is
@@ -361,10 +372,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           int t_o, th, tw;
           conv_tile(p, m_blk, t_o, th, tw);
           const int h0 = th * bh, w0 = tw * bw;
-          const int n0 = n_blk * (SWAP ? BLOCK_M : BLOCK_N);
-          int kcol = 0;
-          for (int kt_ = 0; kt_ < taps_t; ++kt_) {
-            const int t_in = t_o * stride_t + kt_;
+          int n0 = n_blk * (SWAP ? BLOCK_M : BLOCK_N);
+          int taps = taps_t, kcol = 0;
+          if (t_o < p.fold_t) {
+            // folded head: fold rows are [bf16(W0+W1) W2 | bf16(W0+W1+W2)], read from input frame 0 on
+            taps = t_o + 1;
+            kcol = t_o == 0 ? 2 * taps_h * taps_w * cin : 0;
+            n0 += p.fold_n;
+          }
+          for (int kt_ = 0; kt_ < taps; ++kt_) {
+            const int t_in = t_o * stride_t + taps_t - taps + kt_;
             for (int kh_ = 0; kh_ < taps_h; ++kh_) {
               for (int kw_ = 0; kw_ < taps_w; ++kw_) {
                 for (int cb = 0; cb < cin_blocks; ++cb) {
@@ -412,11 +429,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     int mstage = 0;
     uint32_t mphase = 0;
     uint32_t it = 0;
-    auto mainloop = [&](auto&& tail) {
+    auto mainloop = [&](int nkb, auto&& tail) {
       float d[BLOCK_N / 2];
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
-      const int nkb = p.num_k_blocks;
       const bool leader = (threadIdx.x & 127) == 0;
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
@@ -498,7 +514,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       for (int tile = tile0; tile < num_tiles; tile += tile_step, ++it) {
         int m_blk, n_blk;
         tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
-        mainloop([&](float (&d)[BLOCK_N / 2]) { store_tile(d, n_blk); });
+        mainloop(conv_k_blocks(p, m_blk), [&](float (&d)[BLOCK_N / 2]) { store_tile(d, n_blk); });
       }
     } else {
       // The accumulators go to a row-major fp32 tile in shared memory (over the drained operand ring), and the
@@ -546,7 +562,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           fence_proxy_async_smem();
           mbar_arrive(acc_free);
         }
-        mainloop(acc_to_smem);
+        mainloop(conv_k_blocks(p, m_blk), acc_to_smem);
         RowDest dst = row_dest<BLOCK_N>(p, epi, m_blk, n_blk, row, N_COLS);
         const int n_base = n_blk * (KIND == KIND_SWIGLU ? BLOCK_N / 2 : BLOCK_N);   // first output column
 
@@ -1454,7 +1470,10 @@ static int conv3d_impl(const void* x, int T_in_total, int H, int W, int Cin, con
     if (rc) return rc;
   }
   const int K = kt * kh * kw * Cin + (x2 ? C2 : 0);
-  uint64_t db[2] = {(uint64_t)K, (uint64_t)Cout}, sb[1] = {(uint64_t)K * 2};
+  const bool fold = (epi_flags & SVR2_EPI_FOLD_HEAD) != 0;
+  if (fold && (kt != 3 || x2 || Cout % bn))
+    return set_error(SVR2_ERR_ARG, "svr2_conv3d_bf16: SVR2_EPI_FOLD_HEAD needs kt = 3, no shortcut and Cout a multiple of the n-tile");
+  uint64_t db[2] = {(uint64_t)K, (uint64_t)(fold ? 2 * Cout : Cout)}, sb[1] = {(uint64_t)K * 2};
   uint32_t bb[2] = {BLOCK_K, (uint32_t)bn};
   rc = make_tmap_bf16(&tb, w, 2, db, sb, bb);
   if (rc) return rc;
@@ -1492,6 +1511,10 @@ static int conv3d_impl(const void* x, int T_in_total, int H, int W, int Cin, con
   p.out_frame_stride = (long long)H_out * W_out * ldc;
   p.out_t_pad = out_t_pad;
   p.out_dup_head = out_dup_head;
+  if (fold) {
+    p.fold_t = stride_t == 1 ? (T_out < 2 ? T_out : 2) : 1;
+    p.fold_n = Cout;
+  }
   p.bias = (const __nv_bfloat16*)bias;
   p.residual = (const __nv_bfloat16*)residual;
   p.out = y;

@@ -111,11 +111,13 @@ struct Arena {
   size_t need() const { return high + top_used; }
 };
 
-// [pad + T, H, W, C] bf16 activation in the arena; `pad` halo frames in front replicate frame 0 (or hold the previous
-// temporal slice's tail).  stat: GroupNorm partial sums written by the producing conv's epilogue.
+// [pad + T, H, W, C] bf16 activation in the arena; `pad` halo frames in front replicate frame 0 (rep: its producer wrote
+// them so, in the clip's first temporal slice) or hold the previous temporal slice's tail.  stat: GroupNorm partial sums
+// written by the producing conv's epilogue.
 struct Act {
   size_t off = NONE, bytes = 0;
   int T = 0, H = 0, W = 0, C = 0, pad = 0;
+  bool rep = false;
   size_t stat_off = NONE, stat_bytes = 0;
   int slots = 0;
   size_t frame_bytes() const { return (size_t)H * W * C * 2; }
@@ -205,6 +207,7 @@ struct Run {
     const Tensor *g = weight(p + ".weight"), *b = weight(p + ".bias");
     if (!ok()) return y;
     const int dup = pad > 0 && first;
+    y.rep = dup;
     if (x.stat_off != NONE) {
       const size_t cb = (size_t)x.T * x.C * 2 * 4;
       const size_t coef = take(cb);
@@ -244,6 +247,7 @@ struct Run {
     }
     const int Ho = stride_hw == 1 ? x.H : x.H / 2, Wo = stride_hw == 1 ? x.W : x.W / 2;
     Act y = act(T_out, Ho, Wo, Cout, out_pad);
+    y.rep = out_pad > 0 && first;
     const bool with_stats = stats && (Cout == 128 || Cout == 256 || Cout == 512);
     if (with_stats) {
       y.slots = svr2_conv_stat_slots(Cout, Ho, Wo);
@@ -254,24 +258,38 @@ struct Run {
       err(SVR2_ERR_ARG, "svr2_vae: residual shape mismatch");
       return y;
     }
+    const Tensor* wf = x.rep ? head_weight(p + ".weight", kt, Cout, (int64_t)kt * kh * kw * x.C) : nullptr;
     if (dry() || !ok()) return finish_conv(y, p);
     // the kernel indexes the residual with the output's offsets (which include out_pad halo frames)
     const void* res = residual ? P(residual->off) + (size_t)residual->pad * residual->frame_bytes() - (size_t)out_pad * y.frame_bytes()
                                : nullptr;
-    const int epi = SVR2_EPI_BIAS | (residual ? SVR2_EPI_RESIDUAL : 0);
+    const int epi = SVR2_EPI_BIAS | (residual ? SVR2_EPI_RESIDUAL : 0) | (wf ? SVR2_EPI_FOLD_HEAD : 0);
     const int pad_hw = (stride_hw == 1 && kh == 3) ? 1 : 0;
     const int dup = out_pad > 0 && first;
+    const void* wp = wf ? wf->ptr : w->ptr;
     if (with_stats) {
       int slots = 0;
-      ck(svr2_conv3d_stats_bf16(P(x_off), T_in_total, x.H, x.W, x.C, w->ptr, Cout, kt, kh, kw, stride_t, stride_hw, pad_hw,
+      ck(svr2_conv3d_stats_bf16(P(x_off), T_in_total, x.H, x.W, x.C, wp, Cout, kt, kh, kw, stride_t, stride_hw, pad_hw,
                                 T_out, epi, b->ptr, res, P(y.off), out_pad, dup, Cout, P(y.stat_off), (int64_t)y.stat_bytes,
                                 &slots, stream));
       if (ok() && slots != y.slots) err(SVR2_ERR_ARG, "svr2_vae: statistics slot count differs from the plan");
     } else {
-      ck(svr2_conv3d_bf16(P(x_off), T_in_total, x.H, x.W, x.C, w->ptr, Cout, kt, kh, kw, stride_t, stride_hw, pad_hw, T_out,
+      ck(svr2_conv3d_bf16(P(x_off), T_in_total, x.H, x.W, x.C, wp, Cout, kt, kh, kw, stride_t, stride_hw, pad_hw, T_out,
                           epi, b->ptr, res, P(y.off), out_pad, dup, Cout, stream));
     }
     return finish_conv(y, p);
+  }
+  // When the halo in front of a kt = 3 conv's input replicates its frame 0 (Act::rep), output frames 0 and 1 run with the
+  // taps over the copies folded into one weight (SVR2_EPI_FOLD_HEAD).  `name` + ":head" is that weight with the folded
+  // rows appended ([2 Cout, K]); null when it was not loaded.
+  const Tensor* head_weight(const std::string& name, int kt, int Cout, int64_t K) {
+    if (kt != 3 || !ok()) return nullptr;
+    const Tensor* t = find(e, name + ":head");
+    if (t && (t->rank != 2 || t->shape[0] != 2 * (int64_t)Cout || t->shape[1] != K)) {
+      err(SVR2_ERR_ARG, "svr2_vae: folded head weights must be [2 Cout, K]");
+      return nullptr;
+    }
+    return t;
   }
   Act finish_conv(Act& y, const std::string& p) {
     halo(y, p + ":out");
@@ -285,6 +303,7 @@ struct Run {
     const int Cout = (int)w->shape[0], kt = (int)w2->shape[1], kh = (int)w2->shape[2], kw = (int)w2->shape[3], C2 = x.C;
     if (h.pad != kt - 1 || h.T != x.T || h.H != x.H || h.W != x.W || h.C != Cout) { err(SVR2_ERR_ARG, "svr2_vae: fused shortcut shape mismatch"); return Act(); }
     Act y = act(h.T, h.H, h.W, Cout, out_pad);
+    y.rep = out_pad > 0 && first;
     y.slots = svr2_conv_stat_slots(Cout, h.H, h.W);
     y.stat_bytes = (size_t)h.T * y.slots * (Cout / 8) * 16;
     y.stat_off = take(y.stat_bytes);
@@ -421,6 +440,7 @@ struct Run {
     const int z = temporal ? 2 : 1;
     const int T_out = x.T * z - (temporal && first ? 1 : 0);      // remove_head only drops (f=0, z=1) of the clip's first slice
     Act y = act(T_out, 2 * x.H, 2 * x.W, x.C, 2);
+    y.rep = first;
     if (!dry() && ok())
       ck(svr2_upsample_shuffle_bf16(P(x.off) + (size_t)x.pad * x.frame_bytes(), x.T, x.H, x.W, x.C, w->ptr, b->ptr, temporal, first,
                                     P(y.off), 2, first, stream));
@@ -437,6 +457,7 @@ struct Run {
   // T' = 4T-3 for the first slice, else 4T
   void decode_slice(const void* zin, int dt, int64_t zin_cs, int T, int h, int w, void* out, int64_t out_cs, int keep) {
     Act x = act(T, h, w, 64, 2);
+    x.rep = first;
     if (!dry() && ok()) ck(ncdhw_to_ndhwc_strided(zin, dt, 16, T, h, w, zin_cs, P(x.off), 64, 2, 1.0f, stream));
     halo(x, "decoder.in");
     Act c = conv(x, "decoder.conv_in", 0, nullptr, 1, 1, true);

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SVR2_LIB") or os.path.join(HERE, "csrc", "libsvr2.so")   # SVR2_LIB: another build (A/B tools only)
 
 EPI_BIAS, EPI_GATE, EPI_RESIDUAL, EPI_SWIGLU, EPI_GELU, EPI_F32, EPI_SILU = 1, 2, 4, 8, 16, 32, 128
-EPI_ROWSTAT, EPI_PEXP, EPI_ROWSCALE = 256, 512, 1024
+EPI_ROWSTAT, EPI_PEXP, EPI_ROWSCALE, EPI_FOLD_HEAD = 256, 512, 1024, 2048
 
 class ModelDesc(ctypes.Structure):
     """svr2_model_desc (include/svr2.h)"""

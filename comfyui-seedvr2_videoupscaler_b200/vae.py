@@ -32,12 +32,14 @@ from .module import EngineModule
 
 
 class Act:
-    """[pad + T, H, W, C] bf16 activation; ``pad`` halo frames replicate frame 0."""
+    """[pad + T, H, W, C] bf16 activation; ``pad`` halo frames replicate frame 0 (``rep``: its producer wrote them so, in
+    the clip's first temporal slice) or hold the previous slice's tail."""
 
-    def __init__(self, T, H, W, C, pad, device, buf=None):
+    def __init__(self, T, H, W, C, pad, device, buf=None, rep=False):
         self.T, self.H, self.W, self.C, self.pad = T, H, W, C, pad
         self.buf = buf if buf is not None else torch.empty(pad + T, H, W, C, device=device, dtype=torch.bfloat16)
         self.stats = None     # (partial sums tensor, slots) written by the producing conv's epilogue
+        self.rep = rep
 
     @property
     def frame_elems(self):
@@ -78,6 +80,11 @@ class B200VideoVAE(EngineModule):
     # ---- native runtime (csrc/vae_engine.cu): the same sequences in C++ on a svr2_t handle -------------------
     def _device_state_moved(self):
         self._drop_handle()
+        # a device move copies every buffer on its own: make each folded conv's weight a view of its :head rows again
+        W = self.__dict__.get("W")
+        for k in [k for k in W.keys() if k.endswith(":head")] if W is not None else ():
+            head = W[k]
+            self._buffers[W._names[k[: -len(":head")]]] = head[: head.shape[0] // 2]
 
     def _drop_handle(self):
         h = self.__dict__.get("_handle")
@@ -191,10 +198,10 @@ class B200VideoVAE(EngineModule):
         return out
 
     # ---- weights ---------------------------------------------------------
-    def _conv_w(self, w, cin_pad=None, cout_pad=None):
+    def _conv_w(self, w, cin_pad=None, cout_pad=None, dtype=torch.bfloat16):
         """[O,I,kt,kh,kw] -> [O, kt*kh*kw*I] bf16 (K-major, tap-major then channel)."""
         O, I = w.shape[:2]
-        w = w.to(self.device, torch.bfloat16).permute(0, 2, 3, 4, 1)  # O,kt,kh,kw,I
+        w = w.to(self.device, dtype).permute(0, 2, 3, 4, 1)  # O,kt,kh,kw,I
         if cin_pad and cin_pad > I:
             w = torch.nn.functional.pad(w, (0, cin_pad - I))
         w = w.reshape(O, -1)
@@ -247,7 +254,27 @@ class B200VideoVAE(EngineModule):
             W[p + "conv2+shortcut.weight"] = torch.cat([W[p + "conv2.weight"], wsc], 1).contiguous()
             W[p + "conv2+shortcut.bias"] = (W[p + "conv2.bias"].float() + W[p + "conv_shortcut.bias"].float()
                                             ).to(torch.bfloat16).contiguous()
+        # Every kt = 3 conv that runs through svr2_conv3d_bf16 / _stats gets its folded head taps (include/svr2.h
+        # SVR2_EPI_FOLD_HEAD) for the first temporal slice, whose input halo replicates frame 0; the regular weight is the
+        # first Cout rows of that buffer.  (conv2 of a block with a shortcut runs unfolded as conv2+shortcut.)  The sums are
+        # taken over the checkpoint's own weights, so a folded weight is rounded to bf16 once, like each unfolded tap.
+        for k in [k for k in W if k.endswith(".weight")]:
+            if (self.meta.get(k + ".k", (0,))[0] != 3 or k in ("encoder.conv_in.weight", "decoder.conv_out.weight")
+                    or (k.endswith("conv2.weight") and k.replace("conv2.weight", "conv_shortcut.weight") in W)):
+                continue
+            W[k + ":head"] = self._fold_head(self._conv_w(sd[k], cin_pad=64 if k == "decoder.conv_in.weight" else None,
+                                                          dtype=torch.float32))
+            W[k] = W[k + ":head"][: W[k].shape[0]]
         self.W = self._register("w", W)
+
+    @staticmethod
+    def _fold_head(w: torch.Tensor) -> torch.Tensor:
+        """[Cout, 3n] K-major rows of a kt = 3 conv (n = kh*kw*Cin per temporal tap; any float dtype) -> [2 Cout, 3n] bf16:
+        bf16(rows), then [bf16(W0+W1) bf16(W2) | bf16(W0+W1+W2)], the sums in fp32 in that order."""
+        n = w.shape[1] // 3
+        w01, w2 = w[:, :n].float() + w[:, n:2 * n].float(), w[:, 2 * n:].float()
+        fold = torch.cat([w01, w2, w01 + w2], 1)
+        return torch.cat([w, fold], 0).to(torch.bfloat16).contiguous()
 
     # ---- temporal slicing state -------------------------------------------
     @property
@@ -266,7 +293,7 @@ class B200VideoVAE(EngineModule):
 
     # ---- primitive wrappers ----------------------------------------------
     def _gn(self, x: Act, prefix: str, silu: bool, pad: int) -> Act:
-        y = Act(x.T, x.H, x.W, x.C, pad, self.device)
+        y = Act(x.T, x.H, x.W, x.C, pad, self.device, rep=pad > 0 and self._first)
         if x.stats is not None:     # statistics came out of the producing conv's epilogue: finalize + apply only
             part, slots = x.stats
             coef = torch.empty(x.T * x.C * 2, device=self.device, dtype=torch.float32)
@@ -302,15 +329,18 @@ class B200VideoVAE(EngineModule):
         else:
             T_out = (x.T - 1) // stride_t + 1
         Ho, Wo = (x.H, x.W) if stride_hw == 1 else (x.H // 2, x.W // 2)
-        y = Act(T_out, Ho, Wo, w.shape[0], out_pad, self.device)
+        y = Act(T_out, Ho, Wo, w.shape[0], out_pad, self.device, rep=out_pad > 0 and self._first)
         res_ptr = None
         if residual is not None:
             assert (residual.T, residual.H, residual.W, residual.C) == (T_out, Ho, Wo, w.shape[0])
             # the kernel indexes the residual with the output's offsets (which include out_pad halo frames)
             res_ptr = c_void_p(residual.body_ptr() - out_pad * y.frame_elems * 2)
-        epi = lib.EPI_BIAS | (lib.EPI_RESIDUAL if residual is not None else 0)
+        # a halo that replicates frame 0: frames 0 and 1 run folded taps (vae_engine.cu Run::head_weight)
+        wf = self.W.get(prefix + ".weight:head") if (x.rep and kt == 3) else None
+        folded = 0 if wf is None else (3 if stride_t == 1 and T_out >= 2 else 2)      # temporal taps the fold skips
+        epi = lib.EPI_BIAS | (lib.EPI_RESIDUAL if residual is not None else 0) | (lib.EPI_FOLD_HEAD if wf is not None else 0)
         pad_hw = 1 if (stride_hw == 1 and kh == 3) else 0
-        args = (x_ptr, T_in_total, x.H, x.W, x.C, lib.ptr(w), w.shape[0], kt, kh, kw, stride_t, stride_hw,
+        args = (x_ptr, T_in_total, x.H, x.W, x.C, lib.ptr(w if wf is None else wf), w.shape[0], kt, kh, kw, stride_t, stride_hw,
                 pad_hw, T_out, epi, lib.ptr(self.W[prefix + ".bias"]), res_ptr, lib.ptr(y.buf), out_pad,
                 int(out_pad > 0 and self._first), w.shape[0])
         name, extra = "svr2_conv3d_bf16", ()
@@ -321,7 +351,7 @@ class B200VideoVAE(EngineModule):
             y.stats = (part, slots.value)
             name, extra = "svr2_conv3d_stats_bf16", (lib.ptr(part), part.numel() * 4, ctypes.byref(slots))
         lib.call(name, *args, *extra, lib.stream(),
-                 flops=2.0 * T_out * Ho * Wo * self.meta[prefix + ".weight.real"][0] * kt * kh * kw
+                 flops=2.0 * (kt * T_out - folded) * Ho * Wo * self.meta[prefix + ".weight.real"][0] * kh * kw
                  * self.meta[prefix + ".weight.real"][1],
                  tag=(f"|{x.C}>{w.shape[0]}|k{kt}{kh}{kw}|s{stride_t}{stride_hw}|{T_out}x{Ho}x{Wo}"
                       if (lib.PROFILER is not None and lib.PROFILER.detail) else ""))
@@ -344,7 +374,7 @@ class B200VideoVAE(EngineModule):
         kt, kh, kw = self.meta[p + "conv2.weight.k"]
         Cout, C2 = w.shape[0], x.C
         assert h.pad == kt - 1 and (h.T, h.H, h.W) == (x.T, x.H, x.W) and h.C == Cout
-        y = Act(h.T, h.H, h.W, Cout, out_pad, self.device)
+        y = Act(h.T, h.H, h.W, Cout, out_pad, self.device, rep=out_pad > 0 and self._first)
         args = (lib.ptr(h.buf), h.pad + h.T, h.H, h.W, h.C, lib.ptr(w), Cout, kt, kh, kw, h.T, lib.ptr(b),
                 c_void_p(x.body_ptr()), C2, lib.ptr(y.buf), out_pad, int(out_pad > 0 and self._first))
         slots = ctypes.c_int(lib.load().svr2_conv_stat_slots(Cout, h.H, h.W))
@@ -442,13 +472,13 @@ class B200VideoVAE(EngineModule):
         z = 2 if temporal else 1
         first = self._first                       # remove_head only drops (f=0, z=1) of the clip's first slice
         T_out = x.T * z - (1 if temporal and first else 0)
-        y = Act(T_out, 2 * x.H, 2 * x.W, x.C, 2, self.device)
+        y = Act(T_out, 2 * x.H, 2 * x.W, x.C, 2, self.device, rep=first)
         lib.call("svr2_upsample_shuffle_bf16", c_void_p(x.body_ptr()), x.T, x.H, x.W, x.C,
                  lib.ptr(self.W[p + "upscale_conv.weight"]), lib.ptr(self.W[p + "upscale_conv.bias"]), int(temporal),
                  int(first), lib.ptr(y.buf), 2, int(first), lib.stream(),
                  flops=2.0 * x.T * x.H * x.W * x.C * 4 * z * x.C)
         if keep is not None and keep < y.T:
-            y = Act(keep, y.H, y.W, y.C, y.pad, self.device, buf=y.buf[:y.pad + keep])
+            y = Act(keep, y.H, y.W, y.C, y.pad, self.device, buf=y.buf[:y.pad + keep], rep=y.rep)
         self._halo(y, p + "shuffle")
         return self._conv(y, p + "conv", stats=True)
 
@@ -567,7 +597,7 @@ class B200VideoVAE(EngineModule):
         zin = zin.contiguous()
         _, T, h, w = zin.shape
         dt = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}[zin.dtype]
-        x = Act(T, h, w, 64, 2, dev)
+        x = Act(T, h, w, 64, 2, dev, rep=self._first)
         lib.call("svr2_ncdhw_to_ndhwc_bf16", lib.ptr(zin), dt, 16, T, h, w, lib.ptr(x.buf), 64, 2, 1.0, lib.stream())
         self._halo(x, "decoder.in")
         x = self._conv(x, "decoder.conv_in", stats=True)

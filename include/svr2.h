@@ -40,6 +40,7 @@ enum svr2_epilogue {
   SVR2_EPI_ROWSTAT = 256, /* attention pass 1: out[m][slot] = (max, sum exp2) of acc*out_scale over the slot's columns   */
   SVR2_EPI_PEXP = 512,    /* attention pass 2: out = bf16(exp2(acc*out_scale - gate[m])), gate = per-row log2-sum-exp     */
   SVR2_EPI_ROWSCALE = 1024, /* acc * rowscale[m] first (svr2_linear_ex_bf16): un-normalised probabilities x V / row sum   */
+  SVR2_EPI_FOLD_HEAD = 2048, /* svr2_conv3d_bf16 / _stats, kt = 3: folded head taps (see below)                           */
 };
 
 const char* svr2_last_error(void);
@@ -167,6 +168,12 @@ int svr2_linear_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, int
 int svr2_conv3d_bf16(const void* x, int T_in_total, int H, int W, int Cin, const void* w, int Cout, int kt, int kh,
                      int kw, int stride_t, int stride_hw, int pad_hw, int T_out, int epi_flags, const void* bias,
                      const void* residual, void* y, int out_t_pad, int out_dup_head, int ldc, void* stream);
+
+/* SVR2_EPI_FOLD_HEAD (kt = 3): the two halo frames in front of x are copies of its first real frame (the first temporal
+ * slice of a clip).  Output frame 0 then reads [x0 x0 x0] and, for stride_t = 1, frame 1 reads [x0 x0 x1]; they run one
+ * and two temporal taps with weights folded over the copies.  w holds 2 * Cout rows of the same length: rows [0, Cout)
+ * the regular weights [W0 W1 W2], row Cout + co = [bf16(W0+W1) W2 | bf16(W0+W1+W2)], the sums in fp32 in that order.
+ * Cout must be a multiple of the conv's n-tile (128 or 256 for the VAE's convs). */
 
 /* Same conv, additionally emitting per-tile GroupNorm partial sums (fp32, deterministic order) of the stored
  * output so that the following causal_norm_wrapper needs no statistics pass.  stat_partial: [T_out][slots][Cout/8]
