@@ -78,28 +78,6 @@ def test_linear_strided_and_big_k(svr2lib):
     assert_close(out, a.float() @ w.float().T, 4e-3, "strided A")
 
 
-# ------------------------------------------------------------------ attention
-@pytest.mark.parametrize("lens,heads", [([1, 5, 62], 2), ([128, 129, 256], 3), ([400, 868, 63, 810], 2),
-                                        ([2083], 1), ([300] * 9, 20)])
-def test_attn_varlen(svr2lib, lens, heads):
-    total = sum(lens)
-    q, k, v = (bf(rnd(total, heads, 128, seed=s)) for s in (1, 2, 3))
-    cu = torch.tensor([0] + list(torch.tensor(lens).cumsum(0)), dtype=torch.int32, device=DEV)
-    out = svr2lib.attn_varlen(q, k, v, cu, max(lens))
-    ref = torch.empty_like(out, dtype=torch.float32)
-    o = 0
-    for n in lens:
-        qi, ki, vi = (x[o:o + n].float().permute(1, 0, 2) for x in (q, k, v))
-        ref[o:o + n] = F.scaled_dot_product_attention(qi[None], ki[None], vi[None])[0].permute(1, 0, 2)
-        o += n
-    assert_close(out, ref, 1e-2, f"attn {lens}")
-    # fused scatter (window_reverse)
-    perm = torch.randperm(total, device=DEV).int()
-    out2 = torch.zeros_like(out)
-    svr2lib.attn_varlen(q, k, v, cu, max(lens), out=out2, out_row_map=perm)
-    assert torch.equal(out2[perm.long()], out)
-
-
 # ------------------------------------------------------------------ conv3d
 def _to_ndhwc(x_ncdhw, halo):
     x = x_ncdhw[0].permute(1, 2, 3, 0)  # T,H,W,C
@@ -231,49 +209,6 @@ def test_rmsnorm_ada(svr2lib, dim):
     assert_close(out, ref, 3e-3, "mode1")
 
 
-def test_qk_norm_rope_window(svr2lib):
-    heads, L, l, nf = 3, 50, 7, 21
-    inner = heads * 128
-    qkv_v, qkv_t = bf(rnd(L, 3 * inner, seed=1)), bf(rnd(l, 3 * inner, seed=2))
-    wq_v, wk_v, wq_t, wk_t = (rnd(128, seed=s) * 0.1 + 1 for s in (3, 4, 5, 6))
-    R = 40
-    ang = rnd(R, nf, seed=7)
-    cos_t, sin_t = ang.cos().contiguous(), ang.sin().contiguous()
-    g = torch.Generator().manual_seed(0)
-    total = 90
-    src = torch.randint(0, L, (total,), generator=g)
-    is_txt = torch.rand(total, generator=g) < 0.3
-    src = torch.where(is_txt, -(torch.randint(0, l, (total,), generator=g) + 1), src).int().to(DEV)
-    rope = torch.randint(0, R, (total, 3), generator=g).int()
-    rope[::5] = -1
-    rope = rope.to(DEV)
-    q = torch.empty(total, heads, 128, device=DEV, dtype=torch.bfloat16)
-    k, v = torch.empty_like(q), torch.empty_like(q)
-    svr2lib.call("svr2_qk_norm_rope_window_bf16", *(svr2lib.ptr(t) for t in (qkv_v, qkv_t, src, rope.contiguous(),
-                 cos_t, sin_t)), nf, *(svr2lib.ptr(t) for t in (wq_v, wk_v, wq_t, wk_t)), 1e-5, total, heads,
-                 svr2lib.ptr(q), svr2lib.ptr(k), svr2lib.ptr(v), svr2lib.stream())
-    srcl = src.long()
-    rows = torch.where((srcl < 0)[:, None], qkv_t[(-srcl - 1).clamp_min(0)].float(), qkv_v[srcl.clamp_min(0)].float())
-    rows = rows.view(total, 3, heads, 128)
-    for which, (wv, wt), got in ((0, (wq_v, wq_t), q), (1, (wk_v, wk_t), k)):
-        x = rows[:, which]
-        x = x / torch.sqrt(x.pow(2).mean(-1, keepdim=True) + 1e-5)
-        x = x * torch.where((srcl < 0)[:, None, None], wt, wv)
-        c = torch.ones(total, 128, device=DEV)
-        s = torch.zeros(total, 128, device=DEV)
-        for ax in range(3):
-            idx = rope[:, ax].long()
-            cc = torch.where((idx >= 0)[:, None], cos_t[idx.clamp_min(0)], torch.ones(1, device=DEV))
-            ss = torch.where((idx >= 0)[:, None], sin_t[idx.clamp_min(0)], torch.zeros(1, device=DEV))
-            c[:, ax * 2 * nf:(ax + 1) * 2 * nf] = cc.repeat_interleave(2, -1)
-            s[:, ax * 2 * nf:(ax + 1) * 2 * nf] = ss.repeat_interleave(2, -1)
-        x1, x2 = x[..., 0::2], x[..., 1::2]
-        rot = torch.stack((-x2, x1), -1).reshape(x.shape)
-        ref = x * c[:, None] + rot * s[:, None]
-        assert_close(got, ref, 3e-3, "qk" + str(which))
-    assert torch.equal(v.float(), rows[:, 2])
-
-
 @contextlib.contextmanager
 def geometry_handle(svr2lib, variant, heads, freqs, layers=4):
     """A DiT handle that holds nothing but every layer's RoPE frequencies: enough for svr2_dit_geometry."""
@@ -286,49 +221,6 @@ def geometry_handle(svr2lib, variant, heads, freqs, layers=4):
         yield h
     finally:
         svr2lib.engine_destroy(h)
-
-
-@pytest.mark.parametrize("variant,heads,geom", [("3b", 2, (3, 20, 36)), ("3b", 4, (5, 34, 60)), ("7b", 2, (2, 20, 36)),
-                                                ("3b", 20, (1, 10, 14)),
-                                                # full width at the latents of a 4K shard and a 17-frame 1080p clip
-                                                ("3b", 20, (2, 135, 240)), ("7b", 24, (2, 135, 240)),
-                                                ("3b", 20, (5, 68, 120)), ("7b", 24, (5, 68, 120))])
-def test_linear_qkv_rope_fused_vs_unfused(svr2lib, variant, heads, geom):
-    """QKV GEMM with q/k RMSNorm + RoPE + window scatter in its epilogue (svr2_linear_qkv_rope_bf16) + the row-subset
-    kernel for the text rows, against the two-kernel path (svr2_linear_bf16 -> svr2_qk_norm_rope_window_bf16) on the real
-    window layouts (regular and shifted, svr2_dit_geometry): v bit-equal, q/k equal up to the summation order of the
-    per-head RMS."""
-    T, Hp, Wp = geom
-    l, d, inner = 58, heads * 128, heads * 128
-    L = T * Hp * Wp
-    a_v, a_t = bf(rnd(L, d, seed=1)), bf(rnd(l, d, seed=2))
-    w_v, w_t = bf(rnd(3 * inner, d, std=d ** -0.5, seed=3)), bf(rnd(3 * inner, d, std=d ** -0.5, seed=4))
-    nq_v, nk_v, nq_t, nk_t = (rnd(128, seed=s) * 0.1 + 1 for s in (5, 6, 7, 8))
-    nqk = torch.cat([nq_v, nk_v]).contiguous()
-    if variant == "3b":
-        freqs = (1.0 / (10000 ** (torch.arange(0, 42, 2)[:21].float() / 42))).half()
-    else:
-        freqs = (torch.linspace(1.0, 128.0, 10) * math.pi).half()
-    P = svr2lib.ptr
-    with geometry_handle(svr2lib, variant, heads, freqs) as h:
-        for layer in (0, 1):
-            shifted = bool(layer)
-            g = svr2lib.dit_geometry(h, T, 2 * Hp, 2 * Wp, l, layer)
-            rope = (g.rope_cos, g.rope_sin, g.nfreq)
-            qkv_v, qkv_t = svr2lib.linear(a_v, w_v), svr2lib.linear(a_t, w_t)
-            ref = [torch.zeros(g.total, heads, 128, device=DEV, dtype=torch.bfloat16) for _ in range(3)]
-            svr2lib.call("svr2_qk_norm_rope_window_bf16", P(qkv_v), P(qkv_t), g.row_src, g.row_rope, *rope, P(nq_v),
-                         P(nk_v), P(nq_t), P(nk_t), 1e-5, g.total, heads, *(P(t) for t in ref), svr2lib.stream())
-            got = [torch.zeros_like(t) for t in ref]
-            svr2lib.call("svr2_linear_qkv_rope_bf16", P(a_v), d, P(w_v), d, L, heads, d, g.tok_dst, g.tok_rope, *rope,
-                         P(nqk), 1e-5, *(P(t) for t in got), svr2lib.stream())
-            svr2lib.call("svr2_qk_norm_rope_rows_bf16", None, P(qkv_t), g.row_src, g.row_rope, *rope, P(nq_v), P(nk_v),
-                         P(nq_t), P(nk_t), 1e-5, g.txt_rows, g.n_txt_rows, heads, *(P(t) for t in got), svr2lib.stream())
-            assert torch.equal(got[2], ref[2]), "v rows must be bit-equal"
-            for name, g_, r_ in (("q", got[0], ref[0]), ("k", got[1], ref[1])):
-                dlt = (g_.float() - r_.float()).abs()
-                assert (dlt == 0).float().mean() > 0.98 and dlt.max() <= 2 ** -6 * r_.abs().max().item(), \
-                    f"{name} shifted={shifted}: {(dlt == 0).float().mean():.4f} equal, max {dlt.max():.4f}"
 
 
 @pytest.mark.parametrize("variant", ["3b", "7b"])
