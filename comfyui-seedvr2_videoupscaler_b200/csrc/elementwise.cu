@@ -530,17 +530,20 @@ template <> __device__ __forceinline__ float ld_as_float<float>(const float* p, 
 template <> __device__ __forceinline__ float ld_as_float<__nv_bfloat16>(const __nv_bfloat16* p, long long i) { return __bfloat162float(p[i]); }
 template <> __device__ __forceinline__ float ld_as_float<__half>(const __half* p, long long i) { return __half2float(p[i]); }
 
-// in: [C,T,H,W] -> out: [out_t_pad + T, H, W, C_pad] (channels >= C zero), frame 0 duplicated into the halo
+// in: [C,T,H,W] window (channel / frame / row strides in elements) -> out: [out_t_pad + T, H, W, C_pad] (channels >= C
+// zero), frame 0 duplicated into the halo
 template <typename TIn>
 __global__ void ncdhw_to_ndhwc_kernel(const TIn* __restrict__ in, int C, int T, int H, int W, long long chan_stride,
-                                      __nv_bfloat16* __restrict__ out, int C_pad, int out_t_pad, float div) {
+                                      long long frame_stride, int row_stride, __nv_bfloat16* __restrict__ out, int C_pad,
+                                      int out_t_pad, float div) {
   const long long hw = (long long)H * W;
   const long long total = (long long)T * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const long long t = i / hw, pix = i % hw;
+    const long long src = t * frame_stride + (pix / W) * row_stride + pix % W;
     for (int c = 0; c < C_pad; ++c) {
-      const float v = c < C ? bf16_round(ld_as_float<TIn>(in, (long long)c * chan_stride + t * hw + pix)) / div : 0.f;
+      const float v = c < C ? bf16_round(ld_as_float<TIn>(in, (long long)c * chan_stride + src)) / div : 0.f;
       const __nv_bfloat16 b = __float2bfloat16_rn(v);
       out[((t + out_t_pad) * hw + pix) * C_pad + c] = b;
       if (t == 0)
@@ -561,6 +564,56 @@ __global__ void ndhwc_to_ncdhw_kernel(const __nv_bfloat16* __restrict__ in, int 
       if constexpr (sizeof(TOut) == 4) out[(long long)c * chan_stride + t * hw + pix] = v;
       else out[(long long)c * chan_stride + t * hw + pix] = __float2bfloat16_rn(v);
     }
+  }
+}
+
+// ------------------------------------------------------------------ spatially tiled VAE seams
+// The final kernel of a tile accumulates straight into the clip-sized result instead of storing the tile: what
+// svr2_tile_accumulate_bf16 (post.cu tile_accumulate_kernel) does with the stored tile, with the same rounding points —
+// result = bf16(result + rn(rn(v * wh[y]) * ww[x])), count = bf16(fma(wh[y], ww[x], count)) once per pixel.  The edge
+// weights come from the clip's ramp tables (svr2_tile_ramp_bf16: [r | 1 - r]) as vae.py's _tiled builds them: ones,
+// the first ov = min(len, n - 1) entries r on a side with a neighbour before, the last ov entries 1 - r on a side with
+// a neighbour after (which wins where both overlap).
+struct SeamDev {
+  __nv_bfloat16* result;          // at the tile's top-left corner, frame 0 of this call
+  __nv_bfloat16* count;           // at the tile's corner (row stride rs); NULL: not updated
+  long long cs, fs;
+  int rs;
+  const __nv_bfloat16 *ramp_h, *ramp_w;
+  int len_h, len_w, edges;
+};
+__device__ __forceinline__ float seam_weight(const __nv_bfloat16* ramp, int len, bool lo, bool hi, int n, int i) {
+  const int ov = len < n - 1 ? len : n - 1;
+  float w = 1.f;
+  if (ov > 0 && lo && i < ov) w = __bfloat162float(ramp[i]);
+  if (ov > 0 && hi && i >= n - ov) w = __bfloat162float(ramp[len + i - (n - ov)]);
+  return w;
+}
+// v[c]: the tile's bf16 values of pixel (t, y, x) of an H x W tile
+__device__ __forceinline__ void seam_add(const SeamDev& s, int C, const float* v, long long t, int y, int x, int H, int W) {
+  const float a = seam_weight(s.ramp_h, s.len_h, s.edges & SVR2_SEAM_TOP, s.edges & SVR2_SEAM_BOTTOM, H, y);
+  const float b = seam_weight(s.ramp_w, s.len_w, s.edges & SVR2_SEAM_LEFT, s.edges & SVR2_SEAM_RIGHT, W, x);
+  const long long o = t * s.fs + (long long)y * s.rs + x;
+  for (int c = 0; c < C; ++c) {
+    const float u = bf16_round(bf16_round(v[c] * a) * b);
+    __nv_bfloat16* r = s.result + (long long)c * s.cs + o;
+    *r = __float2bfloat16_rn(__bfloat162float(*r) + u);
+  }
+  if (s.count && t == 0) {
+    __nv_bfloat16* k = s.count + (long long)y * s.rs + x;
+    *k = __float2bfloat16_rn(fmaf(a, b, __bfloat162float(*k)));
+  }
+}
+// ndhwc_to_ncdhw_kernel's seam variant (the encoder's 16 mean channels of conv_out)
+__global__ void __launch_bounds__(256) ndhwc_to_ncdhw_seam_kernel(const __nv_bfloat16* __restrict__ in, int ld_in, int C,
+                                                                  int T, int H, int W, SeamDev s) {
+  const long long hw = (long long)H * W, total = (long long)T * hw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long t = i / hw, pix = i % hw;
+    float v[16];
+    for (int c = 0; c < C; ++c) v[c] = __bfloat162float(in[i * ld_in + c]);
+    seam_add(s, C, v, t, (int)(pix / W), (int)(pix % W), H, W);
   }
 }
 
@@ -637,6 +690,25 @@ __global__ void __launch_bounds__(256) im2col3_kernel(const __nv_bfloat16* __res
 // Decoder conv_out (128 -> 3, 3x3x3 causal) as (1) one GEMM z[tap*co_n + co][pixel] = W_tap[co,:] . x[pixel,:]
 // over ALL input pixels incl. the 2 halo frames (x is read once instead of 27 times), fp32, and (2) this
 // gather: out[co][t][h][w] = bias[co] + sum_taps z[tap, co][(t+kt), h+kh-1, w+kw-1] (zero outside the frame).
+__device__ __forceinline__ void conv_tap_sum(const float* __restrict__ z, long long ldz, int co_n, int H, int W,
+                                             long long t, int h, int w, float* acc) {
+  const long long hw = (long long)H * W;
+#pragma unroll
+  for (int kt = 0; kt < 3; ++kt)
+#pragma unroll
+    for (int kh = 0; kh < 3; ++kh) {
+      const int hh = h + kh - 1;
+      if (hh < 0 || hh >= H) continue;
+#pragma unroll
+      for (int kw = 0; kw < 3; ++kw) {
+        const int ww = w + kw - 1;
+        if (ww < 0 || ww >= W) continue;
+        const long long q = (t + kt) * hw + (long long)hh * W + ww;     // halo: input frame index = t + kt
+        const int tap = (kt * 3 + kh) * 3 + kw;
+        for (int c = 0; c < co_n; ++c) acc[c] += z[(long long)(tap * co_n + c) * ldz + q];
+      }
+    }
+}
 template <typename TOut>
 __global__ void __launch_bounds__(256) conv_tap_gather_kernel(const float* __restrict__ z, long long ldz, int co_n,
                                                               const __nv_bfloat16* __restrict__ bias, int T, int H, int W,
@@ -647,26 +719,27 @@ __global__ void __launch_bounds__(256) conv_tap_gather_kernel(const float* __res
     const int w = i % W, h = (i / W) % H;
     const long long t = i / hw;
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int kt = 0; kt < 3; ++kt)
-#pragma unroll
-      for (int kh = 0; kh < 3; ++kh) {
-        const int hh = h + kh - 1;
-        if (hh < 0 || hh >= H) continue;
-#pragma unroll
-        for (int kw = 0; kw < 3; ++kw) {
-          const int ww = w + kw - 1;
-          if (ww < 0 || ww >= W) continue;
-          const long long q = (t + kt) * hw + (long long)hh * W + ww;     // halo: input frame index = t + kt
-          const int tap = (kt * 3 + kh) * 3 + kw;
-          for (int c = 0; c < co_n; ++c) acc[c] += z[(long long)(tap * co_n + c) * ldz + q];
-        }
-      }
+    conv_tap_sum(z, ldz, co_n, H, W, t, h, w, acc);
     for (int c = 0; c < co_n; ++c) {
       const float v = bf16_round(acc[c] + __bfloat162float(bias[c]));
       if constexpr (sizeof(TOut) == 4) out[(long long)c * chan_stride + i] = v;
       else out[(long long)c * chan_stride + i] = __float2bfloat16_rn(v);
     }
+  }
+}
+// conv_tap_gather_kernel's seam variant (the decoder's last kernel): v = bf16(bias + sum over the taps), accumulated
+__global__ void __launch_bounds__(256) conv_tap_gather_seam_kernel(const float* __restrict__ z, long long ldz, int co_n,
+                                                                   const __nv_bfloat16* __restrict__ bias, int T, int H,
+                                                                   int W, SeamDev s) {
+  const long long hw = (long long)H * W, total = (long long)T * hw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int w = i % W, h = (i / W) % H;
+    const long long t = i / hw;
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    conv_tap_sum(z, ldz, co_n, H, W, t, h, w, acc);
+    for (int c = 0; c < co_n; ++c) acc[c] = bf16_round(acc[c] + __bfloat162float(bias[c]));
+    seam_add(s, co_n, acc, t, h, w, H, W);
   }
 }
 
@@ -831,19 +904,26 @@ extern "C" int svr2_transpose_bf16(const void* in, int64_t ld_in, void* out, int
   return check_launch("transpose");
 }
 
-// channel stride of the NCDHW side in elements (T*H*W for a contiguous tensor; larger for a temporal slice of a clip)
-int svr2::ncdhw_to_ndhwc_strided(const void* in, int in_dtype, int C, int T, int H, int W, int64_t chan_stride, void* out,
-                                 int C_pad, int out_t_pad, float div, void* stream) {
+// strides of the NCDHW side in elements: a rectangle of a clip's frames (a spatial tile) or all of them
+int svr2::ncdhw_to_ndhwc_window(const void* in, int in_dtype, int C, int T, int H, int W, int64_t chan_stride,
+                                int64_t frame_stride, int row_stride, void* out, int C_pad, int out_t_pad, float div,
+                                void* stream) {
   const long long total = (long long)T * H * W;
   int blocks = (int)((total + 255) / 256);
   if (blocks > 132 * 16) blocks = 132 * 16;
   cudaStream_t s = (cudaStream_t)stream;
-  const long long cs = chan_stride;
-  if (in_dtype == 0) ncdhw_to_ndhwc_kernel<float><<<blocks, 256, 0, s>>>((const float*)in, C, T, H, W, cs, (__nv_bfloat16*)out, C_pad, out_t_pad, div);
-  else if (in_dtype == 1) ncdhw_to_ndhwc_kernel<__nv_bfloat16><<<blocks, 256, 0, s>>>((const __nv_bfloat16*)in, C, T, H, W, cs, (__nv_bfloat16*)out, C_pad, out_t_pad, div);
-  else if (in_dtype == 2) ncdhw_to_ndhwc_kernel<__half><<<blocks, 256, 0, s>>>((const __half*)in, C, T, H, W, cs, (__nv_bfloat16*)out, C_pad, out_t_pad, div);
+  const long long cs = chan_stride, fs = frame_stride;
+  const int rs = row_stride;
+  if (in_dtype == 0) ncdhw_to_ndhwc_kernel<float><<<blocks, 256, 0, s>>>((const float*)in, C, T, H, W, cs, fs, rs, (__nv_bfloat16*)out, C_pad, out_t_pad, div);
+  else if (in_dtype == 1) ncdhw_to_ndhwc_kernel<__nv_bfloat16><<<blocks, 256, 0, s>>>((const __nv_bfloat16*)in, C, T, H, W, cs, fs, rs, (__nv_bfloat16*)out, C_pad, out_t_pad, div);
+  else if (in_dtype == 2) ncdhw_to_ndhwc_kernel<__half><<<blocks, 256, 0, s>>>((const __half*)in, C, T, H, W, cs, fs, rs, (__nv_bfloat16*)out, C_pad, out_t_pad, div);
   else return set_error(SVR2_ERR_ARG, "ncdhw_to_ndhwc: dtype must be 0 (f32), 1 (bf16) or 2 (f16)");
   return check_launch("ncdhw_to_ndhwc");
+}
+// channel stride of the NCDHW side in elements (T*H*W for a contiguous tensor; larger for a temporal slice of a clip)
+int svr2::ncdhw_to_ndhwc_strided(const void* in, int in_dtype, int C, int T, int H, int W, int64_t chan_stride, void* out,
+                                 int C_pad, int out_t_pad, float div, void* stream) {
+  return ncdhw_to_ndhwc_window(in, in_dtype, C, T, H, W, chan_stride, (int64_t)H * W, W, out, C_pad, out_t_pad, div, stream);
 }
 extern "C" int svr2_ncdhw_to_ndhwc_bf16(const void* in, int in_dtype, int C, int T, int H, int W, void* out, int C_pad,
                                         int out_t_pad, float div, void* stream) {
@@ -900,4 +980,54 @@ int svr2::conv_tap_gather_strided(const float* z, int64_t ldz, int co_n, const v
 extern "C" int svr2_conv_tap_gather(const float* z, int64_t ldz, int co_n, const void* bias, int T, int H, int W,
                                     void* out, int out_dtype, void* stream) {
   return conv_tap_gather_strided(z, ldz, co_n, bias, T, H, W, out, out_dtype, (int64_t)T * H * W, stream);
+}
+
+static SeamDev seam_dev(const svr2::Seam& s) {
+  return SeamDev{(__nv_bfloat16*)s.result, (__nv_bfloat16*)s.count, (long long)s.cs, (long long)s.fs, s.rs,
+                 (const __nv_bfloat16*)s.ramp_h, (const __nv_bfloat16*)s.ramp_w, s.len_h, s.len_w, s.edges};
+}
+static int seam_check(const svr2::Seam& s, const char* what) {
+  if (!s.result || (s.len_h > 0 && !s.ramp_h) || (s.len_w > 0 && !s.ramp_w) || s.len_h < 0 || s.len_w < 0) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "%s: result NULL, or a ramp table of positive length NULL", what);
+    return set_error(SVR2_ERR_ARG, buf);
+  }
+  return SVR2_OK;
+}
+int svr2::conv_tap_gather_seam(const float* z, int64_t ldz, int co_n, const void* bias, int T, int H, int W, const Seam& s,
+                               void* stream) {
+  if (co_n < 1 || co_n > 4) return set_error(SVR2_ERR_ARG, "conv_tap_gather_seam: 1 <= co_n <= 4");
+  if (int rc = seam_check(s, "conv_tap_gather_seam")) return rc;
+  const long long total = (long long)T * H * W;
+  if (total <= 0) return SVR2_OK;
+  long long blocks = (total + 255) / 256;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
+  conv_tap_gather_seam_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(z, ldz, co_n, (const __nv_bfloat16*)bias,
+                                                                                   T, H, W, seam_dev(s));
+  return check_launch("conv_tap_gather_seam");
+}
+int svr2::ndhwc_to_ncdhw_seam(const void* in, int ld_in, int C, int T, int H, int W, const Seam& s, void* stream) {
+  if (C < 1 || C > 16 || ld_in < C) return set_error(SVR2_ERR_ARG, "ndhwc_to_ncdhw_seam: 1 <= C <= 16, ld_in >= C");
+  if (int rc = seam_check(s, "ndhwc_to_ncdhw_seam")) return rc;
+  const long long total = (long long)T * H * W;
+  if (total <= 0) return SVR2_OK;
+  int blocks = (int)((total + 255) / 256);
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  ndhwc_to_ncdhw_seam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)in, ld_in, C, T, H, W,
+                                                                       seam_dev(s));
+  return check_launch("ndhwc_to_ncdhw_seam");
+}
+extern "C" int svr2_conv_tap_gather_seam_bf16(const float* z, int64_t ldz, int co_n, const void* bias, int T, int H, int W,
+                                              void* result, int64_t chan_stride, int64_t frame_stride, int row_stride,
+                                              void* count, const void* ramp_h, int len_h, const void* ramp_w, int len_w,
+                                              int edges, void* stream) {
+  const Seam s{result, chan_stride, frame_stride, row_stride, count, ramp_h, ramp_w, len_h, len_w, edges};
+  return conv_tap_gather_seam(z, ldz, co_n, bias, T, H, W, s, stream);
+}
+extern "C" int svr2_ndhwc_to_ncdhw_seam_bf16(const void* in, int ld_in, int C, int T, int H, int W, void* result,
+                                             int64_t chan_stride, int64_t frame_stride, int row_stride, void* count,
+                                             const void* ramp_h, int len_h, const void* ramp_w, int len_w, int edges,
+                                             void* stream) {
+  const Seam s{result, chan_stride, frame_stride, row_stride, count, ramp_h, ramp_w, len_h, len_w, edges};
+  return ndhwc_to_ncdhw_seam(in, ld_in, C, T, H, W, s, stream);
 }

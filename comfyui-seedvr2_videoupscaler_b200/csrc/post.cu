@@ -367,6 +367,28 @@ __global__ void __launch_bounds__(256) tile_normalize_kernel(__nv_bfloat16* __re
     result[i] = __float2bfloat16_rn(__bfloat162float(result[i]) / c);
   }
 }
+// ramp(n) of vae.py's _tiled on the device: torch.linspace(0, 1, n, dtype=bf16) on CUDA (ATen's kernel in bf16
+// arithmetic: step = bf16(1 / bf16(n - 1)); entry i < n / 2 is 0 + step * bf16(i), the rest 1 - step * bf16(n - 1 - i),
+// every product and sum rounded), then * pi, cos, * 0.5, 0.5 - (each rounded), and 1 - r behind it
+__device__ __forceinline__ float tile_ramp_value(int n, int i) {
+  float t = 0.f;
+  if (n > 1) {
+    const float step = rn(1.0f / rn((float)(n - 1)));
+    t = i < n / 2 ? rn(0.0f + rn(step * rn((float)i))) : rn(1.0f - rn(step * rn((float)(n - 1 - i))));
+  }
+  const float c = rn(cosf(rn(t * (float)M_PI)));
+  return rn(0.5f - rn(0.5f * c));
+}
+__global__ void __launch_bounds__(256) tile_ramp_kernel(__nv_bfloat16* __restrict__ rh, int nh, __nv_bfloat16* __restrict__ rw,
+                                                        int nw) {
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < nh + nw; i += gridDim.x * 256) {
+    __nv_bfloat16* out = i < nh ? rh : rw;
+    const int n = i < nh ? nh : nw, j = i < nh ? i : i - nh;
+    const float r = tile_ramp_value(n, j);
+    out[j] = __float2bfloat16_rn(r);
+    out[n + j] = __float2bfloat16_rn(1.0f - r);
+  }
+}
 
 inline int grid_for(long long n, int per_block = 256, int waves = 16) {
   long long b = (n + per_block - 1) / per_block;
@@ -579,4 +601,17 @@ extern "C" int svr2_tile_normalize_bf16(void* result, const void* count, int pla
   tile_normalize_kernel<<<grid_for((long long)planes * hw), 256, 0, (cudaStream_t)stream>>>(
       (__nv_bfloat16*)result, (const __nv_bfloat16*)count, planes, hw);
   return check_launch("tile_normalize");
+}
+
+int svr2::tile_ramp(void* ramp_h, int len_h, void* ramp_w, int len_w, void* stream) {
+  if (len_h < 0 || len_w < 0 || (len_h > 0 && !ramp_h) || (len_w > 0 && !ramp_w))
+    return set_error(SVR2_ERR_ARG, "svr2_tile_ramp_bf16: lengths >= 0, tables of positive length not NULL");
+  const int n = len_h + len_w;
+  if (n == 0) return SVR2_OK;
+  tile_ramp_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)ramp_h, len_h, (__nv_bfloat16*)ramp_w,
+                                                                     len_w);
+  return check_launch("tile_ramp");
+}
+extern "C" int svr2_tile_ramp_bf16(void* ramp_h, int len_h, void* ramp_w, int len_w, void* stream) {
+  return tile_ramp(ramp_h, len_h, ramp_w, len_w, stream);
 }

@@ -19,6 +19,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
+#include <array>
 #include <string>
 #include <unordered_map>
 #include <utility>
@@ -108,7 +110,13 @@ struct Arena {
     top_used += bytes;
     return cap - top_used;
   }
-  size_t need() const { return high + top_used; }
+  size_t peak = 0;                // high + top_used before the last release_top()
+  // the whole top region is free again (the next spatial tile starts its own slicing state)
+  void release_top() {
+    if (high + top_used > peak) peak = high + top_used;
+    top_used = 0;
+  }
+  size_t need() const { return high + top_used > peak ? high + top_used : peak; }
 };
 
 // [pad + T, H, W, C] bf16 activation in the arena; `pad` halo frames in front replicate frame 0 (rep: its producer wrote
@@ -123,6 +131,39 @@ struct Act {
   size_t frame_bytes() const { return (size_t)H * W * C * 2; }
 };
 
+// The tile plan of tiled_encode / tiled_decode as vae.py's _tiled computes it.  encode: H x W sample pixels; decode:
+// H x W latent pixels.  Tiles are latent rectangles [y0, y1) x [x0, x1) in row-major order.
+struct TilePlan {
+  bool encode = false, whole = false;     // whole: the frame fits one tile, the pass runs un-tiled
+  int Hl = 0, Wl = 0, s = 1;              // latent frame; result pixels per latent pixel
+  int ovh = 0, ovw = 0;                   // ramp lengths in result pixels
+  std::vector<std::array<int, 4>> tiles;
+};
+TilePlan tile_plan(bool encode, int H, int W, int tile_h, int tile_w, int overlap_h, int overlap_w) {
+  TilePlan p;
+  const int f = 8;
+  const int th = tile_h / f > 1 ? tile_h / f : 1, tw = tile_w / f > 1 ? tile_w / f : 1;
+  p.encode = encode;
+  p.whole = encode ? (H <= tile_h && W <= tile_w) : (H <= th && W <= tw);
+  const int loh = std::max(0, std::min(overlap_h / f, th - 1)), low = std::max(0, std::min(overlap_w / f, tw - 1));
+  const int sh = std::max(1, th - loh), sw = std::max(1, tw - low);
+  p.Hl = encode ? (H + f - 1) / f : H;
+  p.Wl = encode ? (W + f - 1) / f : W;
+  p.s = encode ? 1 : f;
+  p.ovh = encode ? loh : overlap_h;
+  p.ovw = encode ? low : overlap_w;
+  if (p.whole) return p;
+  for (int y0 = 0; y0 < p.Hl; y0 += sh) {
+    const int y1 = std::min(y0 + th, p.Hl);
+    for (int x0 = 0; x0 < p.Wl; x0 += sw) {
+      const int x1 = std::min(x0 + tw, p.Wl);
+      if ((y0 > 0 && y1 - y0 <= loh) || (x0 > 0 && x1 - x0 <= low)) continue;    // inside the previous tile's overlap
+      p.tiles.push_back({y0, y1, x0, x1});
+    }
+  }
+  return p;
+}
+
 struct Run {
   svr2_engine* e;
   Arena A;
@@ -133,6 +174,14 @@ struct Run {
   std::unordered_map<std::string, size_t> state;     // layer key -> top-region offset of the previous slice's tail
   int64_t launches = 0;
   int rc = SVR2_OK;
+  // while a spatially tiled pass runs one tile: the input is a window of the clip (strides in elements) and the final
+  // kernel is the seam variant, accumulating into the clip-sized result (seam.result: the tile's corner, frame 0)
+  struct TileIO {
+    int64_t in_cs, in_fs;
+    int in_rs;
+    Seam seam;
+  };
+  const TileIO* tile = nullptr;
 
   Run(svr2_engine* eng, size_t cap, char* b, void* st) : e(eng), A(cap), base(b), stream(st) {}
   bool dry() const { return base == nullptr; }
@@ -458,7 +507,7 @@ struct Run {
   void decode_slice(const void* zin, int dt, int64_t zin_cs, int T, int h, int w, void* out, int64_t out_cs, int keep) {
     Act x = act(T, h, w, 64, 2);
     x.rep = first;
-    if (!dry() && ok()) ck(ncdhw_to_ndhwc_strided(zin, dt, 16, T, h, w, zin_cs, P(x.off), 64, 2, 1.0f, stream));
+    if (!dry() && ok()) ck(read_input(zin, dt, 16, T, h, w, zin_cs, P(x.off), 64));
     halo(x, "decoder.in");
     Act c = conv(x, "decoder.conv_in", 0, nullptr, 1, 1, true);
     drop(x);
@@ -487,7 +536,8 @@ struct Run {
     if (!dry() && ok()) {
       if (npix > 0x7fffffffLL) err(SVR2_ERR_ARG, "svr2_vae_decode: slice too large (pixels per slice must fit 31 bits)");
       linear(wt->ptr, g.C, P(g.off), g.C, 81, (int)npix, g.C, SVR2_EPI_F32, nullptr, nullptr, nullptr, P(z), ldz, 1.f);
-      if (ok()) ck(conv_tap_gather_strided((const float*)P(z), ldz, 3, bo->ptr, g.T, g.H, g.W, out, 1, out_cs, stream));
+      if (ok() && tile) ck(conv_tap_gather_seam((const float*)P(z), ldz, 3, bo->ptr, g.T, g.H, g.W, seam_at(out), stream));
+      else if (ok()) ck(conv_tap_gather_strided((const float*)P(z), ldz, 3, bo->ptr, g.T, g.H, g.W, out, 1, out_cs, stream));
     }
     give(z, z_b);
     drop(g);
@@ -497,7 +547,7 @@ struct Run {
   // T = 1 + 4k for the first slice (T' = k + 1), 4k afterwards (T' = k)
   void encode_slice(const void* xin, int dt, int64_t xin_cs, int T, int H, int W, void* out, int64_t out_cs) {
     Act x8 = act(T, H, W, 8, 2);
-    if (!dry() && ok()) ck(ncdhw_to_ndhwc_strided(xin, dt, 3, T, H, W, xin_cs, P(x8.off), 8, 2, 1.0f, stream));
+    if (!dry() && ok()) ck(read_input(xin, dt, 3, T, H, W, xin_cs, P(x8.off), 8));
     halo(x8, "encoder.in");
     const size_t col_b = (size_t)T * H * W * 128 * 2;
     const size_t col = take(col_b);
@@ -528,8 +578,23 @@ struct Run {
     drop(h);
     Act c = conv(g, "encoder.conv_out", 0, nullptr, 1, 1, false);
     drop(g);
-    if (!dry() && ok()) ck(ndhwc_to_ncdhw_strided(P(c.off), c.C, 16, c.T, c.H, c.W, out, 1, out_cs, stream));
+    if (!dry() && ok() && tile) ck(ndhwc_to_ncdhw_seam(P(c.off), c.C, 16, c.T, c.H, c.W, seam_at(out), stream));
+    else if (!dry() && ok()) ck(ndhwc_to_ncdhw_strided(P(c.off), c.C, 16, c.T, c.H, c.W, out, 1, out_cs, stream));
     drop(c);
+  }
+
+  // the input conversion of a slice: the whole clip's frames, or the current tile's window of them
+  int read_input(const void* in, int dt, int C, int T, int H, int W, int64_t cs, void* out, int C_pad) {
+    if (tile) return ncdhw_to_ndhwc_window(in, dt, C, T, H, W, cs, tile->in_fs, tile->in_rs, out, C_pad, 2, 1.0f, stream);
+    return ncdhw_to_ndhwc_strided(in, dt, C, T, H, W, cs, out, C_pad, 2, 1.0f, stream);
+  }
+  // the current tile's seam at `out` (this slice's first frame); the count plane takes each pixel's weight once, in the
+  // first slice
+  Seam seam_at(void* out) const {
+    Seam s = tile->seam;
+    s.result = out;
+    if (!first) s.count = nullptr;
+    return s;
   }
 
   // slicing_decode (attn_video_vae.py:1279-1300): the first slice is latent frame 0 plus `size` frames, then `size` each.
@@ -537,7 +602,8 @@ struct Run {
   // decode-then-crop returns the same values.  Slices past them do not run, the last one that does is trimmed.
   void decode(const void* z, int dt, int T, int h, int w, int size, int frames, void* out) {
     const int esz = dt == 0 ? 4 : 2;
-    const int64_t zin_cs = (int64_t)T * h * w, out_cs = (int64_t)frames * 64 * h * w;
+    const int64_t zin_cs = tile ? tile->in_cs : (int64_t)T * h * w, out_cs = (int64_t)frames * 64 * h * w;
+    const int64_t in_fs = tile ? tile->in_fs : (int64_t)h * w, out_fs = tile ? tile->seam.fs : (int64_t)64 * h * w;
     if (size <= 0 || T - 1 <= size) {
       decode_slice(z, dt, zin_cs, T, h, w, out, out_cs, frames);
       return;
@@ -549,7 +615,7 @@ struct Run {
       const int keep = frames - o0 < n_out ? frames - o0 : n_out;
       if (keep <= 0) break;                // this and every later slice lie past the wanted frames
       tails = o0 + n_out < frames;         // a later slice runs and continues from this one's tails
-      decode_slice((const char*)z + (size_t)a * h * w * esz, dt, zin_cs, b - a, h, w, (char*)out + (size_t)o0 * 64 * h * w * 2,
+      decode_slice((const char*)z + (size_t)a * in_fs * esz, dt, zin_cs, b - a, h, w, (char*)out + (size_t)o0 * out_fs * 2,
                    out_cs, keep);
     }
   }
@@ -559,7 +625,8 @@ struct Run {
   void encode(const void* x, int dt, int T, int H, int W, int size, void* out) {
     const int esz = dt == 0 ? 4 : 2;
     const int T_lat = (T - 1) / 4 + 1;
-    const int64_t xin_cs = (int64_t)T * H * W, out_cs = (int64_t)T_lat * (H / 8) * (W / 8);
+    const int64_t xin_cs = tile ? tile->in_cs : (int64_t)T * H * W, out_cs = (int64_t)T_lat * (H / 8) * (W / 8);
+    const int64_t in_fs = tile ? tile->in_fs : (int64_t)H * W, out_fs = tile ? tile->seam.fs : (int64_t)(H / 8) * (W / 8);
     if (size <= 0 || T - 1 <= size || (T - 1) % 4 != 0) {
       encode_slice(x, dt, xin_cs, T, H, W, out, out_cs);
       return;
@@ -569,9 +636,55 @@ struct Run {
     for (int a = 0, b = 1 + size; a < T && ok(); a = b, b = (b + size < T ? b + size : T)) {
       first = a == 0;
       const int64_t o0 = a == 0 ? 0 : (a - 1) / 4 + 1;
-      encode_slice((const char*)x + (size_t)a * H * W * esz, dt, xin_cs, b - a, H, W,
-                   (char*)out + (size_t)o0 * (H / 8) * (W / 8) * 2, out_cs);
+      encode_slice((const char*)x + (size_t)a * in_fs * esz, dt, xin_cs, b - a, H, W, (char*)out + (size_t)o0 * out_fs * 2,
+                   out_cs);
     }
+  }
+
+  // tiled_encode / tiled_decode (attn_video_vae.py:1302-1630) in vae.py _tiled's order: the frame is cut into latent
+  // tiles of tile // 8 stepping by tile // 8 - overlap // 8, a tile wholly inside the previous one's overlap is skipped;
+  // each tile runs the whole (temporally sliced) encoder / decoder with its own slicing state on a window of the clip,
+  // and its final kernel accumulates it into `out` with the edge weights; `out` is normalised by the count plane at the
+  // end.  encode: x [3, T, H, W] -> [16, T', H/8, W/8]; decode: z [16, T, H, W] -> [3, frames, 8H, 8W].
+  void tiled(const TilePlan& p, const void* in, int dt, int T, int H, int W, int size, int frames, void* out) {
+    const int esz = dt == 0 ? 4 : 2, f = p.encode ? 8 : 1;        // input pixels per latent pixel
+    const int C = p.encode ? 16 : 3, T_out = p.encode ? (T - 1) / 4 + 1 : frames;
+    const int Hr = p.Hl * p.s, Wr = p.Wl * p.s;
+    const size_t plane = (size_t)Hr * Wr, count_b = plane * 2;
+    const size_t count = take(count_b);
+    const size_t rh_b = (size_t)4 * p.ovh, rw_b = (size_t)4 * p.ovw;
+    const size_t rh = p.ovh > 0 ? take(rh_b) : NONE, rw = p.ovw > 0 ? take(rw_b) : NONE;
+    if (!dry() && ok()) {
+      if (!dev_zero(out, (size_t)C * T_out * count_b, stream) || !dev_zero(P(count), count_b, stream))
+        err(SVR2_ERR_CUDA, "svr2_vae: memset failed");
+      ck(tile_ramp(rh == NONE ? nullptr : P(rh), p.ovh, rw == NONE ? nullptr : P(rw), p.ovw, stream));
+    }
+    for (const auto& r : p.tiles) {
+      if (!ok()) break;
+      const int y0 = r[0], y1 = r[1], x0 = r[2], x1 = r[3];
+      const size_t corner = ((size_t)y0 * p.s * Wr + (size_t)x0 * p.s) * 2;
+      TileIO io;
+      io.in_cs = (int64_t)T * H * W;
+      io.in_fs = (int64_t)H * W;
+      io.in_rs = W;
+      io.seam = Seam{(char*)out + corner, (int64_t)T_out * (int64_t)plane, (int64_t)plane, Wr, dry() ? nullptr : P(count) + corner,
+                     rh == NONE ? nullptr : P(rh), rw == NONE ? nullptr : P(rw), p.ovh, p.ovw,
+                     (y0 > 0 ? SVR2_SEAM_TOP : 0) | (y1 < p.Hl ? SVR2_SEAM_BOTTOM : 0) | (x0 > 0 ? SVR2_SEAM_LEFT : 0) |
+                         (x1 < p.Wl ? SVR2_SEAM_RIGHT : 0)};
+      tile = &io;
+      slicing = false;
+      first = tails = true;
+      state.clear();
+      A.release_top();
+      const char* src = (const char*)in + ((size_t)y0 * f * W + (size_t)x0 * f) * esz;
+      if (p.encode) encode(src, dt, T, (y1 - y0) * 8, (x1 - x0) * 8, size, io.seam.result);
+      else decode(src, dt, T, y1 - y0, x1 - x0, size, frames, io.seam.result);
+      tile = nullptr;
+    }
+    if (!dry() && ok()) ck(svr2_tile_normalize_bf16(out, P(count), C * T_out, (int64_t)plane, stream));
+    give(rw, rw_b);
+    give(rh, rh_b);
+    give(count, count_b);
   }
 };
 
@@ -597,17 +710,34 @@ int check_frames(svr2_engine* e, const char* what, int T, int frames) {
   return fail(e, SVR2_ERR_ARG, buf);
 }
 
+// a spatial tile of at least one pixel, overlaps >= 0
+int check_tiles(svr2_engine* e, const char* what, int tile_h, int tile_w, int overlap_h, int overlap_w) {
+  if (tile_h >= 1 && tile_w >= 1 && overlap_h >= 0 && overlap_w >= 0) return SVR2_OK;
+  char buf[160];
+  snprintf(buf, sizeof buf, "%s: tile sizes >= 1 and overlaps >= 0 (got %d x %d, %d x %d)", what, tile_h, tile_w, overlap_h,
+           overlap_w);
+  return fail(e, SVR2_ERR_ARG, buf);
+}
+
+// the whole pass on one Run: spatially tiled when `tiles` cuts the frame, else un-tiled
+void sequence(Run& r, const TilePlan* tiles, int encode, const void* in, int dt, int T, int H, int W, int slice_frames,
+              int frames, void* out) {
+  if (tiles && !tiles->whole) r.tiled(*tiles, in, dt, T, H, W, slice_frames, frames, out);
+  else if (encode) r.encode(in, dt, T, H, W, slice_frames, out);
+  else r.decode(in, dt, T, H, W, slice_frames, frames, out);
+}
+
 // frames: output frames of a decode (ignored by an encode)
-size_t plan_bytes(svr2_engine* e, int encode, int T, int H, int W, int slice_frames, int frames) {
+size_t plan_bytes(svr2_engine* e, int encode, int T, int H, int W, int slice_frames, int frames, const TilePlan* tiles = nullptr) {
   Run r(e, ~(size_t)0 / 2, nullptr, nullptr);
-  if (encode) r.encode(nullptr, 1, T, H, W, slice_frames, nullptr);
-  else r.decode(nullptr, 1, T, H, W, slice_frames, frames, nullptr);
+  sequence(r, tiles, encode, nullptr, 1, T, H, W, slice_frames, frames, nullptr);
   return r.ok() ? r.A.need() : 0;
 }
 
 int run(svr2_engine* e, int encode, const void* in, int dt, int T, int H, int W, int slice_frames, int frames, void* out,
-        void* ws, size_t ws_bytes, void* stream) {
-  const char* what = encode ? "svr2_vae_encode" : "svr2_vae_decode";
+        void* ws, size_t ws_bytes, void* stream, const TilePlan* tiles = nullptr) {
+  const char* what = tiles ? (encode ? "svr2_vae_encode_tiled" : "svr2_vae_decode_tiled")
+                           : (encode ? "svr2_vae_encode" : "svr2_vae_decode");
   int rc = check_args(e, what, T, H, W, encode ? 8 : 1);
   if (!rc && !encode) rc = check_frames(e, what, T, frames);
   if (rc) return rc;
@@ -618,7 +748,7 @@ int run(svr2_engine* e, int encode, const void* in, int dt, int T, int H, int W,
   cudaGetDevice(&cur);
   if (cur != e->device) return fail(e, SVR2_ERR_ARG, "svr2_vae: the handle's device is not the current device");
 #endif
-  const size_t need = plan_bytes(e, encode, T, H, W, slice_frames, frames);
+  const size_t need = plan_bytes(e, encode, T, H, W, slice_frames, frames, tiles);
   if (!need) return SVR2_ERR_ARG;      // message already recorded
   if (!e->vae) e->vae = new VaeState();
   char* base;
@@ -642,8 +772,7 @@ int run(svr2_engine* e, int encode, const void* in, int dt, int T, int H, int W,
     base = (char*)v->workspace;
   }
   Run r(e, need, base, stream);
-  if (encode) r.encode(in, dt, T, H, W, slice_frames, out);
-  else r.decode(in, dt, T, H, W, slice_frames, frames, out);
+  sequence(r, tiles, encode, in, dt, T, H, W, slice_frames, frames, out);
   e->vae->last_launches = r.launches;
   return r.rc;
 }
@@ -680,6 +809,33 @@ extern "C" int svr2_vae_decode(svr2_t* e, const void* z, int z_dtype, int T, int
 extern "C" int svr2_vae_decode_frames(svr2_t* e, const void* z, int z_dtype, int T, int h, int w, int slice_frames, int frames,
                                       void* sample, void* workspace, size_t workspace_bytes, void* stream) {
   return run(e, 0, z, z_dtype, T, h, w, slice_frames, frames, sample, workspace, workspace_bytes, stream);
+}
+
+// Spatially tiled passes (see svr2.h): the same arguments as the un-tiled ones plus the tile plan's four settings
+extern "C" size_t svr2_vae_tiled_workspace_bytes(svr2_t* e, int direction, int T, int H, int W, int tile_h, int tile_w,
+                                                 int overlap_h, int overlap_w, int slice_frames, int frames) {
+  const char* what = "svr2_vae_tiled_workspace_bytes";
+  if (check_args(e, what, T, H, W, direction == 0 ? 8 : 1) || check_tiles(e, what, tile_h, tile_w, overlap_h, overlap_w) ||
+      (direction != 0 && check_frames(e, what, T, frames)))
+    return 0;
+  const TilePlan p = tile_plan(direction == 0, H, W, tile_h, tile_w, overlap_h, overlap_w);
+  return plan_bytes(e, direction == 0, T, H, W, slice_frames, frames, &p);
+}
+
+extern "C" int svr2_vae_encode_tiled(svr2_t* e, const void* x, int x_dtype, int T, int H, int W, int tile_h, int tile_w,
+                                     int overlap_h, int overlap_w, int slice_frames, void* latent, void* workspace,
+                                     size_t workspace_bytes, void* stream) {
+  if (int rc = check_tiles(e, "svr2_vae_encode_tiled", tile_h, tile_w, overlap_h, overlap_w)) return rc;
+  const TilePlan p = tile_plan(true, H, W, tile_h, tile_w, overlap_h, overlap_w);
+  return run(e, 1, x, x_dtype, T, H, W, slice_frames, 0, latent, workspace, workspace_bytes, stream, &p);
+}
+
+extern "C" int svr2_vae_decode_tiled(svr2_t* e, const void* z, int z_dtype, int T, int h, int w, int tile_h, int tile_w,
+                                     int overlap_h, int overlap_w, int slice_frames, int frames, void* sample,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  if (int rc = check_tiles(e, "svr2_vae_decode_tiled", tile_h, tile_w, overlap_h, overlap_w)) return rc;
+  const TilePlan p = tile_plan(false, h, w, tile_h, tile_w, overlap_h, overlap_w);
+  return run(e, 0, z, z_dtype, T, h, w, slice_frames, frames, sample, workspace, workspace_bytes, stream, &p);
 }
 
 // kernels launched by the last svr2_vae_encode / svr2_vae_decode of this handle (bench.py's gpu_launches)

@@ -53,6 +53,11 @@ SIGNATURES = {
     "svr2_vae_decode": [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
     "svr2_vae_decode_frames_workspace_bytes": [_P, c_int, c_int, c_int, c_int, c_int],
     "svr2_vae_decode_frames": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, ctypes.c_size_t, _P],
+    "svr2_vae_tiled_workspace_bytes": [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int],
+    "svr2_vae_encode_tiled": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P,
+                              ctypes.c_size_t, _P],
+    "svr2_vae_decode_tiled": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P,
+                              ctypes.c_size_t, _P],
     "svr2_vae_last_launches": [_P],
     "svr2_linear_bf16": [_P, c_int64, _P, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int64, c_float, _P],
     "svr2_conv3d_bf16": [_P, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
@@ -104,6 +109,11 @@ SIGNATURES = {
     "svr2_blend_overlap_f32": [_P, _P, _P, _P, _P, c_int, c_int64, _P],
     "svr2_tile_accumulate_bf16": [_P, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P],
     "svr2_tile_normalize_bf16": [_P, _P, c_int, c_int64, _P],
+    "svr2_tile_ramp_bf16": [_P, c_int, _P, c_int, _P],
+    "svr2_conv_tap_gather_seam_bf16": [_P, c_int64, c_int, _P, c_int, c_int, c_int, _P, c_int64, c_int64, c_int, _P, _P,
+                                       c_int, _P, c_int, c_int, _P],
+    "svr2_ndhwc_to_ncdhw_seam_bf16": [_P, c_int, c_int, c_int, c_int, c_int, _P, c_int64, c_int64, c_int, _P, _P, c_int,
+                                      _P, c_int, c_int, _P],
     "svr2_resize_scratch_bytes": [c_int, c_int, c_int, c_int],
     "svr2_resize_bicubic_aa_bf16": [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P, c_int64,
                                     _P],

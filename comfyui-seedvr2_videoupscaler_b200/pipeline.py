@@ -24,7 +24,7 @@ import torch
 
 from . import alpha, color_fix, noise as gen_noise, preprocess
 from .dit import B200NaDiT, dit_config
-from .vae import B200VideoVAE
+from .vae import B200VideoVAE, tile_settings
 
 SCALING_FACTOR = 0.9152   # configs_3b/main.yaml:60
 SHIFTING_FACTOR = 0.0
@@ -56,6 +56,28 @@ def pad_video_temporal(frames: torch.Tensor, count: int = 0, prepend: bool = Fal
     return torch.cat([rev, frames] if prepend else [frames, rev], 0)
 
 
+# The VAE loader's spatial tiling settings (encode_tiled / decode_tiled with *_tile_size / *_tile_overlap in sample
+# pixels, an int or an (h, w) pair each) and their defaults.  Tiling changes results by design, so it is never on by itself.
+TILING = dict(encode_tiled=False, encode_tile_size=1024, encode_tile_overlap=128,
+              decode_tiled=False, decode_tile_size=1024, decode_tile_overlap=128)
+
+
+def tiling_settings(tiling: dict) -> dict:
+    """The six tiling settings given (names checked), {} when neither pass is tiled: the phases then take the same
+    calls as without them."""
+    unknown = set(tiling) - set(TILING)
+    if unknown:
+        raise TypeError(f"unknown tiling settings {sorted(unknown)}; expected {sorted(TILING)}")
+    t = dict(TILING, **tiling)
+    return t if (t["encode_tiled"] or t["decode_tiled"]) else {}
+
+
+def _tiles(tiling: dict, phase: str):
+    """(tile_h, tile_w, overlap_h, overlap_w) of ``phase`` ("encode" / "decode"), None when it is not tiled."""
+    t = dict(TILING, **tiling)
+    return tile_settings(t[phase + "_tile_size"], t[phase + "_tile_overlap"]) if t[phase + "_tiled"] else None
+
+
 def _frames_kw(phase, frames: int) -> dict:
     """``{"frames": frames}`` for a phase method (``vae_decode``, ``clip_workspace``) that takes the decoded frame count;
     ``{}`` for a replacement with the plain signature, which then decodes (plans) every frame and the caller crops."""
@@ -75,9 +97,11 @@ class SeedVR2Engine:
 
     # ---- VideoDiffusionInfer.vae_encode ---------------------------------
     @torch.no_grad()
-    def vae_encode(self, clip: torch.Tensor, workspace=None) -> torch.Tensor:
-        """clip (3,T,H,W) in [-1,1] -> latent (T',h,w,16) bf16, scaled."""
-        z = self.vae.encode(clip[None].to(self.device, torch.bfloat16), workspace=workspace).latent   # (1,16,T',h,w)
+    def vae_encode(self, clip: torch.Tensor, workspace=None, tiles: Optional[tuple] = None) -> torch.Tensor:
+        """clip (3,T,H,W) in [-1,1] -> latent (T',h,w,16) bf16, scaled.  ``tiles``: (tile_h, tile_w, overlap_h,
+        overlap_w) of a spatially tiled encode."""
+        tkw = {} if tiles is None else dict(tiled=True, tile_size=tiles[:2], tile_overlap=tiles[2:])
+        z = self.vae.encode(clip[None].to(self.device, torch.bfloat16), workspace=workspace, **tkw).latent   # (1,16,T',h,w)
         z = (z - SHIFTING_FACTOR) * SCALING_FACTOR
         return z[0].permute(1, 2, 3, 0).contiguous()
 
@@ -102,27 +126,32 @@ class SeedVR2Engine:
 
     # ---- VideoDiffusionInfer.vae_decode -----------------------------------
     @torch.no_grad()
-    def vae_decode(self, latent: torch.Tensor, workspace=None, frames: Optional[int] = None) -> torch.Tensor:
+    def vae_decode(self, latent: torch.Tensor, workspace=None, frames: Optional[int] = None,
+                   tiles: Optional[tuple] = None) -> torch.Tensor:
         """latent (T',h,w,16) -> sample (3,T,H,W) bf16 in ~[-1,1]; ``frames``: only the first ``frames`` of the T = 4T'-3
-        frames are decoded (the same values; None: all)."""
+        frames are decoded (the same values; None: all).  ``tiles``: as in ``vae_encode``."""
         z = latent.permute(3, 0, 1, 2)[None]
         z = z / SCALING_FACTOR + SHIFTING_FACTOR
-        return self.vae.decode(z, workspace=workspace, frames=frames).sample[0]
+        tkw = {} if tiles is None else dict(tiled=True, tile_size=tiles[:2], tile_overlap=tiles[2:])
+        return self.vae.decode(z, workspace=workspace, frames=frames, **tkw).sample[0]
 
-    def clip_workspace(self, T: int, Hp: int, Wp: int, frames: Optional[int] = None) -> Optional[torch.Tensor]:
+    def clip_workspace(self, T: int, Hp: int, Wp: int, frames: Optional[int] = None, **tiling) -> Optional[torch.Tensor]:
         """ONE workspace for the three phases of a clip of T (4n+1) frames at Hp x Wp (multiples of 16) of which the first
         ``frames`` are decoded (None: all): the maximum of the exact needs of VAE encode, the DiT forward and VAE decode
-        (svr2_vae_workspace_bytes / svr2_workspace_bytes / svr2_vae_decode_frames_workspace_bytes), with the VAE passes
-        temporally sliced until they fit the free HBM.  The phases run one after the other on one stream, so they can
-        share the bytes; the block is the engine's resident workspace (lib.workspace: kept between clips, grown on demand;
-        the capture pool inside a CUDA graph).  None when a phase runs on the Python sequencing (profiling)."""
+        (svr2_vae_workspace_bytes / svr2_workspace_bytes / svr2_vae_decode_frames_workspace_bytes, or
+        svr2_vae_tiled_workspace_bytes for a pass that ``tiling`` — the six settings of ``TILING`` — tiles), with the VAE
+        passes temporally sliced until they fit the free HBM.  The phases run one after the other on one stream, so they
+        can share the bytes; the block is the engine's resident workspace (lib.workspace: kept between clips, grown on
+        demand; the capture pool inside a CUDA graph).  None when a phase runs on the Python sequencing (profiling)."""
         from . import lib
+        tiling_settings(tiling)
         if not (self.vae._use_native() and self.dit.native and lib.PROFILER is None):
             return None
         Tl, h, w = (T - 1) // 4 + 1, Hp // 8, Wp // 8
         budget = int(0.92 * self.vae._free_bytes()) - 2 * 3 * T * Hp * Wp * 2      # the decoded clip and its crop
-        need = max(self.vae.plan_slices(True, T, Hp, Wp, budget)[1],
-                   self.vae.plan_slices(False, Tl, h, w, budget, frames=frames)[1],
+        enc, dec = _tiles(tiling, "encode"), _tiles(tiling, "decode")
+        need = max(self.vae.plan_slices(True, T, Hp, Wp, budget, **({} if enc is None else {"tiles": enc}))[1],
+                   self.vae.plan_slices(False, Tl, h, w, budget, frames=frames, **({} if dec is None else {"tiles": dec}))[1],
                    self.dit.workspace_bytes(Tl, h, w, self.txt.shape[0]))
         return lib.workspace(need, self.device)
 
@@ -153,19 +182,20 @@ class SeedVR2Engine:
                      color_correction: str = "none", resolution: Optional[int] = None,
                      max_resolution: int = 0, keep_alpha: bool = False, input_noise_scale: float = 0.0,
                      latent_noise_scale: float = 0.0, input_noise: Optional[torch.Tensor] = None,
-                     latent_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     latent_noise: Optional[torch.Tensor] = None, **tiling) -> torch.Tensor:
         """frames (T,h,w,3) in [0,1]; ``resolution`` = target shortest edge (None: keep the size, i.e. the frames
         are already at the target resolution).  Returns (T,H,W,3) bf16 in [0,1] on the device.
         ``color_correction``: "none", "lab" (the reference CLI default), "wavelet", "adain" or "wavelet_adaptive" —
         matched against the transformed input clip (generation_phases.py:1299-1317).
         ``keep_alpha``: frames (T,h,w,4) are RGBA; returns (T,H,W,4) with the alpha upscaled against the decoded RGB
         (generation_phases.py:1142-1217).  Without it a 4th channel is ignored.
-        ``input_noise_scale``, ``latent_noise_scale``, ``input_noise``, ``latent_noise``: see ``clip_to_sample``."""
+        ``input_noise_scale``, ``latent_noise_scale``, ``input_noise``, ``latent_noise`` and the spatial tiling settings
+        (``encode_tiled`` …): see ``clip_to_sample``."""
         rgba = keep_alpha and frames.shape[-1] == 4
         out = self.clip_to_sample(frames, noise=noise, seed=seed, resolution=resolution, max_resolution=max_resolution,
                                   keep_alpha=rgba, input_noise_scale=input_noise_scale,
                                   latent_noise_scale=latent_noise_scale, input_noise=input_noise,
-                                  latent_noise=latent_noise)
+                                  latent_noise=latent_noise, **tiling)
         return self.finish_clip(*out, color_correction=color_correction)
 
     @staticmethod
@@ -196,7 +226,7 @@ class SeedVR2Engine:
                        resolution: Optional[int] = None, max_resolution: int = 0, keep_alpha: bool = False,
                        input_noise_scale: float = 0.0, latent_noise_scale: float = 0.0,
                        input_noise: Optional[torch.Tensor] = None, latent_noise: Optional[torch.Tensor] = None,
-                       input_generator: Optional[torch.Generator] = None):
+                       input_generator: Optional[torch.Generator] = None, **tiling):
         """Phases 1-3 for one clip: frames (T,h,w,3) in [0,1] -> (sample, style), both (T,3,H,W) bf16 in [-1,1]:
         the decoded clip and the transformed input clip it is colour-matched against in phase 4.  ``keep_alpha``
         (frames (T,h,w,4)): (sample, style, src) with src the input frames on the device, unpadded, whose alpha
@@ -207,7 +237,14 @@ class SeedVR2Engine:
         ``input_generator``, else from a fresh generator seeded ``seed + 1_000_000`` (the reference's first batch).
         ``latent_noise_scale`` > 0: the DiT condition is augmented (:679-704) with ``latent_noise`` (T',h,w,16) when
         given, else with a second draw of the DiT noise generator right after ``noise``; an explicit ``noise`` needs
-        an explicit ``latent_noise``.  Both scales must be finite and >= 0; at 0 nothing extra is drawn."""
+        an explicit ``latent_noise``.  Both scales must be finite and >= 0; at 0 nothing extra is drawn.
+
+        Spatial tiling, the VAE loader's settings (``TILING``): ``encode_tiled`` / ``decode_tiled`` run that VAE pass in
+        tiles of ``*_tile_size`` sample pixels overlapping by ``*_tile_overlap`` (an int or an (h, w) pair; defaults
+        1024 / 128), cross-faded at the seams — a different result by design, in a workspace that no longer grows
+        with the frame area (a 9-frame 4K batch on one 80 GB GPU).  Off by default; off, the phases run as without them."""
+        tiling = tiling_settings(tiling)
+        enc_tiles, dec_tiles = _tiles(tiling, "encode"), _tiles(tiling, "decode")
         input_noise_scale = gen_noise.check_scale("input_noise_scale", input_noise_scale)
         latent_noise_scale = gen_noise.check_scale("latent_noise_scale", latent_noise_scale)
         if latent_noise_scale > 0 and noise is not None and latent_noise is None:
@@ -222,7 +259,7 @@ class SeedVR2Engine:
         H0, W0 = tf.true_size(frames.shape[1], frames.shape[2])
         x = tf.run(x, channels_last=True)                           # (3, T, Hp, Wp) bf16 in [-1,1]
         # only the T0 real frames are decoded: the padding frames' decoder work after its last temporal upsampler is skipped
-        ws = self.clip_workspace(x.shape[1], x.shape[2], x.shape[3], **_frames_kw(self.clip_workspace, T0))
+        ws = self.clip_workspace(x.shape[1], x.shape[2], x.shape[3], **_frames_kw(self.clip_workspace, T0), **tiling)
         kw = {} if ws is None else {"workspace": ws}
         x_enc = x
         if input_noise_scale > 0:
@@ -231,7 +268,7 @@ class SeedVR2Engine:
                 layout = self.input_noise_layout(frames, resolution, max_resolution)
                 input_noise = gen_noise.draw_input_noise(x.shape, g, self.device, layout)
             x_enc = gen_noise.add_input_noise(x, input_noise, input_noise_scale)
-        latent = self.vae_encode(x_enc, **kw)
+        latent = self.vae_encode(x_enc, **kw, **({} if enc_tiles is None else {"tiles": enc_tiles}))
         del x_enc
         if noise is None:
             g = torch.Generator(device=self.device).manual_seed(seed)
@@ -240,7 +277,8 @@ class SeedVR2Engine:
                 latent_noise = gen_noise.draw_latent_noise(latent.shape, g, self.device)
         aug = dict(latent_noise=latent_noise, latent_noise_scale=latent_noise_scale) if latent_noise_scale > 0 else {}
         x0 = self.inference(noise, latent, **kw, **aug)
-        y = self.vae_decode(x0, **kw, **_frames_kw(self.vae_decode, T0))      # (3,T0,H,W), or (3,T,H,W)
+        y = self.vae_decode(x0, **kw, **_frames_kw(self.vae_decode, T0),
+                            **({} if dec_tiles is None else {"tiles": dec_tiles}))      # (3,T0,H,W), or (3,T,H,W)
         del ws, kw
         sample = y[:, :T0, :H0, :W0].permute(1, 0, 2, 3)            # t c h w, the layout of phase 4
         style = x[:, :T0, :H0, :W0].permute(1, 0, 2, 3)            # the transformed input clip in [-1,1]
@@ -251,7 +289,7 @@ class SeedVR2Engine:
                       color_correction: str = "none", resolution: Optional[int] = None,
                       max_resolution: int = 0, keep_alpha: bool = False, input_noise_scale: float = 0.0,
                       latent_noise_scale: float = 0.0, uniform_batch_size: bool = False,
-                      prepend_frames: int = 0) -> torch.Tensor:
+                      prepend_frames: int = 0, **tiling) -> torch.Tensor:
         """A whole video on one GPU the way the reference's four phases do it (generation_phases.py:271-289, 344-358,
         969-1000, 1236-1345): batches of ``batch_size`` frames stepping by ``batch_size - temporal_overlap``, every batch
         seeded identically, the overlap cross-faded into the previous batch's tail, colour correction per batch
@@ -267,10 +305,11 @@ class SeedVR2Engine:
         output (generation_utils.py:196-198, generation_phases.py:1388-1397).  A multi-GPU caller prepends once,
         before sharding.  Each slice is post-processed as soon as it is final (``final_slices``), so the device holds
         the result and fewer than ``batch_size + temporal_overlap`` decoded frames; ``stream_video`` hands the slices
-        to the host instead."""
+        to the host instead.  ``tiling``: the spatial tiling settings of ``clip_to_sample``, for every batch."""
         slices = [s for done in self._final_slices(frames, batch_size, temporal_overlap, seed, color_correction,
                                                    resolution, max_resolution, keep_alpha, input_noise_scale,
-                                                   latent_noise_scale, uniform_batch_size, prepend_frames)
+                                                   latent_noise_scale, uniform_batch_size, prepend_frames,
+                                                   tiling=tiling_settings(tiling))
                   for s in done]
         out = torch.cat(slices, 0)
         if 0 < prepend_frames < out.shape[0]:
@@ -282,7 +321,7 @@ class SeedVR2Engine:
                      color_correction: str = "none", resolution: Optional[int] = None, max_resolution: int = 0,
                      keep_alpha: bool = False, input_noise_scale: float = 0.0, latent_noise_scale: float = 0.0,
                      uniform_batch_size: bool = False, prepend_frames: int = 0,
-                     out_dtype: torch.dtype = torch.uint8) -> Iterator[Tuple[int, torch.Tensor]]:
+                     out_dtype: torch.dtype = torch.uint8, **tiling) -> Iterator[Tuple[int, torch.Tensor]]:
         """``upscale_video`` for videos of any length: device memory does not grow with the video.  ``frames``: one
         (T,h,w,C) tensor or an iterable of (t,h,w,C) chunks of any sizes, on the host or the device (a decoder's
         output, read only as far as the next batch needs; float in [0,1] or the reference CLI's uint8 RGB frames).
@@ -290,7 +329,8 @@ class SeedVR2Engine:
         each (t,H,W,C) in pinned host memory (torch's caching host allocator) that the caller owns.  C is 3, or 4
         with ``keep_alpha`` and RGBA input.  ``out_dtype``: ``torch.uint8``, the CLI's 8-bit frames
         (``(video.float() * 255.0).astype(np.uint8)`` of ``upscale_video``'s result), or ``torch.bfloat16``, that
-        result itself.  The other options are those of ``upscale_video``, with the same result frame for frame.
+        result itself.  The other options, the spatial tiling settings included, are those of ``upscale_video``, with
+        the same result frame for frame.
 
         On the engine's one stream, every batch is enqueued first, then the cross-fade, phase 4 and the copy to the
         host of the slices it made final, followed by an event; only then does the host wait for the copies enqueued
@@ -300,6 +340,7 @@ class SeedVR2Engine:
         is known that more follow (the reference keeps all frames when p is not smaller than the output)."""
         if out_dtype not in (torch.uint8, torch.bfloat16):
             raise ValueError(f"out_dtype must be torch.uint8 or torch.bfloat16, got {out_dtype}")
+        tiling = tiling_settings(tiling)
         cuda = self.device.type == "cuda"
         p = prepend_frames
         state = dict(seen=0, index=0)          # output frames so far (before the drop), frames yielded
@@ -338,7 +379,7 @@ class SeedVR2Engine:
         prev = None
         for done in self._final_slices(frames, batch_size, temporal_overlap, seed, color_correction, resolution,
                                        max_resolution, keep_alpha, input_noise_scale, latent_noise_scale,
-                                       uniform_batch_size, prepend_frames, out_dtype):
+                                       uniform_batch_size, prepend_frames, out_dtype, tiling=tiling):
             cur = to_host(done)
             del done
             if prev is not None:
@@ -356,7 +397,7 @@ class SeedVR2Engine:
 
     def _final_slices(self, frames, batch_size, temporal_overlap, seed, color_correction, resolution, max_resolution,
                       keep_alpha, input_noise_scale, latent_noise_scale, uniform_batch_size, prepend_frames,
-                      out_dtype=torch.bfloat16):
+                      out_dtype=torch.bfloat16, tiling=None):
         """``final_slices`` over the engine's batches: per batch, the phase-4 images (on the device) it made final."""
         from . import shard
         input_noise_scale = gen_noise.check_scale("input_noise_scale", input_noise_scale)
@@ -373,7 +414,7 @@ class SeedVR2Engine:
             if uniform_batch_size and b - a < batch_size:
                 batch = pad_video_temporal(batch, count=batch_size - (b - a))
             out = self.clip_to_sample(batch, seed=seed, resolution=resolution, max_resolution=max_resolution,
-                                      keep_alpha=rgba, **noise_kw)
+                                      keep_alpha=rgba, **noise_kw, **(tiling or {}))
             s, st = out[0][:b - a].contiguous(), out[1][:b - a].contiguous()
             return (s, (st, out[2][:b - a])) if rgba else (s, st)
 

@@ -53,6 +53,17 @@ class Act:
         return self.buf[self.pad:]
 
 
+def tile_settings(tile_size, tile_overlap) -> tuple:
+    """(tile_h, tile_w, overlap_h, overlap_w) in sample pixels from a spatial tile size and overlap, each an int or an
+    (h, w) pair (the VAE loader's ``*_tile_size`` / ``*_tile_overlap``)."""
+    def pair(v, name, lo):
+        h, w = (v, v) if isinstance(v, int) else tuple(v)
+        if int(h) != h or int(w) != w or h < lo or w < lo:
+            raise ValueError(f"{name} must be an int >= {lo} or a pair of them, got {v!r}")
+        return int(h), int(w)
+    return pair(tile_size, "tile_size", 1) + pair(tile_overlap, "tile_overlap", 0)
+
+
 class VAEOutput:
     def __init__(self, **kw):
         self.__dict__.update(kw)
@@ -127,16 +138,20 @@ class B200VideoVAE(EngineModule):
         return tensors
 
     def workspace_bytes(self, encode: bool, T: int, H: int, W: int, slice_frames: int = 0,
-                        frames: Optional[int] = None) -> int:
+                        frames: Optional[int] = None, tiles: Optional[tuple] = None) -> int:
         """Exact workspace of one native encode (T sample frames of H x W) / decode (T latent frames of H x W latent
         pixels) with temporal slices of ``slice_frames`` (0 = un-sliced); ``frames``: the decoded frames wanted (None:
-        all 4T-3)."""
+        all 4T-3); ``tiles``: (tile_h, tile_w, overlap_h, overlap_w) of a spatially tiled pass (None: un-tiled)."""
         frames = None if encode else (4 * T - 3 if frames is None else frames)
-        key = (bool(encode), T, H, W, slice_frames, frames)
+        key = (bool(encode), T, H, W, slice_frames, frames, tiles)
         if key not in self._ws_bytes:
             L, h = lib.load(), self.native_handle()
-            n = int(L.svr2_vae_workspace_bytes(h, 0, T, H, W, slice_frames) if encode
-                    else L.svr2_vae_decode_frames_workspace_bytes(h, T, H, W, slice_frames, frames))
+            if tiles is not None:
+                n = int(L.svr2_vae_tiled_workspace_bytes(h, 0 if encode else 1, T, H, W, *tiles, slice_frames,
+                                                         0 if encode else frames))
+            else:
+                n = int(L.svr2_vae_workspace_bytes(h, 0, T, H, W, slice_frames) if encode
+                        else L.svr2_vae_decode_frames_workspace_bytes(h, T, H, W, slice_frames, frames))
             if n <= 0:
                 raise lib.Svr2Error("svr2_vae workspace query failed: " + L.svr2_engine_last_error(h).decode())
             self._ws_bytes[key] = n
@@ -152,16 +167,19 @@ class B200VideoVAE(EngineModule):
         return free + torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device) + held
 
     def plan_slices(self, encode: bool, T: int, H: int, W: int, budget: Optional[int] = None,
-                    frames: Optional[int] = None):
+                    frames: Optional[int] = None, tiles: Optional[tuple] = None):
         """(slice_frames, workspace bytes) of a native encode (T sample frames of H x W) / decode (T latent frames of
         H x W latent pixels; ``frames``: the decoded frames wanted, None: all): the longest temporal slice — un-sliced
         first, then set_causal_slicing's split, then shorter ones — whose EXACT workspace fits ``budget`` bytes (default:
-        92 % of the free HBM incl. torch's cached blocks)."""
+        92 % of the free HBM incl. torch's cached blocks).  ``tiles``: (tile_h, tile_w, overlap_h, overlap_w) — the
+        same search for a spatially tiled pass, whose every tile is sliced alike."""
         step = 4 if encode else 1
         cap = None if self.split_size is None else (max(4, self.split_size // 4 * 4) if encode else max(1, self.split_size // 4))
         can_slice = not (encode and (T - 1) % 4)       # only 4n+1-frame clips continue the temporal stride phase
         sz = 0 if (cap is None or T - 1 <= cap or not can_slice) else cap
         fr = {} if frames is None else {"frames": frames}
+        if tiles is not None:
+            fr["tiles"] = tiles
         need = self.workspace_bytes(encode, T, H, W, sz, **fr)
         if can_slice:
             if budget is None:
@@ -175,20 +193,28 @@ class B200VideoVAE(EngineModule):
         return sz, need
 
     def _native_run(self, encode: bool, src: torch.Tensor, T: int, H: int, W: int, out: torch.Tensor, workspace=None,
-                    frames: Optional[int] = None):
+                    frames: Optional[int] = None, tiles: Optional[tuple] = None):
         """``workspace``: a uint8 CUDA tensor shared by the phases of a clip (pipeline.SeedVR2Engine.clip_workspace) or None —
         then the engine's resident block (lib.workspace; the capture pool inside a CUDA graph).  ``frames``: decode only
-        the first ``frames`` output frames (None: all)."""
+        the first ``frames`` output frames (None: all).  ``tiles``: (tile_h, tile_w, overlap_h, overlap_w), a spatially
+        tiled pass (svr2_vae_encode_tiled / svr2_vae_decode_tiled)."""
         if workspace is not None:
-            sz, need = self.plan_slices(encode, T, H, W, budget=workspace.numel(), frames=frames)
+            sz, need = self.plan_slices(encode, T, H, W, budget=workspace.numel(), frames=frames, tiles=tiles)
             if need > workspace.numel():
                 raise lib.Svr2Error(f"B200VideoVAE: workspace of {workspace.numel()} bytes given, {need} needed")
             ws = workspace
         else:
-            sz, need = self.plan_slices(encode, T, H, W, frames=frames)
+            sz, need = self.plan_slices(encode, T, H, W, frames=frames, tiles=tiles)
             ws = lib.workspace(need, self.device)
         dt = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}[src.dtype]
-        if encode:
+        if tiles is not None:
+            if encode:
+                lib.call("svr2_vae_encode_tiled", self.native_handle(), lib.ptr(src), dt, T, H, W, *tiles, sz, lib.ptr(out),
+                         lib.ptr(ws), ws.numel(), lib.stream())
+            else:
+                lib.call("svr2_vae_decode_tiled", self.native_handle(), lib.ptr(src), dt, T, H, W, *tiles, sz,
+                         4 * T - 3 if frames is None else frames, lib.ptr(out), lib.ptr(ws), ws.numel(), lib.stream())
+        elif encode:
             lib.call("svr2_vae_encode", self.native_handle(), lib.ptr(src), dt, T, H, W, sz, lib.ptr(out), lib.ptr(ws),
                      ws.numel(), lib.stream())
         else:
@@ -557,7 +583,9 @@ class B200VideoVAE(EngineModule):
                frames: Optional[int] = None):
         """z (1,16,T,h,w) or (1,16,h,w) -> .sample (1,3,4T-3,8h,8w) bf16 (Decoder3D.forward).  ``frames``: return only
         the first ``frames`` (1 .. 4T-3) output frames, the same values; the decoder is causal in time, so the layers
-        after the last temporal upsampler run on those frames alone (the spatially tiled decode decodes all and crops)."""
+        after the last temporal upsampler run on those frames alone.  ``tiled``: spatial tiles of ``tile_size`` sample
+        pixels overlapping by ``tile_overlap`` (each an int or an (h, w) pair; default 512 / 64), see ``_tiled``; on
+        the native runtime by default (svr2_vae_decode_tiled)."""
         self._require_cuda("B200VideoVAE.decode")
         squeeze = z.ndim == 4
         if squeeze:
@@ -566,9 +594,14 @@ class B200VideoVAE(EngineModule):
         if frames is not None and not 1 <= frames <= 4 * T - 3:
             raise ValueError(f"frames = {frames}: a decode of {T} latent frames returns 1 .. {4 * T - 3} frames")
         if tiled:
-            out = self._tiled(z, False, tile_size or (512, 512), tile_overlap or (64, 64))
-            if frames is not None:
-                out = out[:, :, :frames]
+            tiles = tile_settings(tile_size or 512, 64 if tile_overlap is None else tile_overlap)
+            if self._use_native():
+                _, _, T, h, w = z.shape
+                F = 4 * T - 3 if frames is None else frames
+                out = torch.empty(1, 3, F, 8 * h, 8 * w, device=self.device, dtype=torch.bfloat16)
+                self._native_run(False, z[0].to(self.device).contiguous(), T, h, w, out, workspace, frames=F, tiles=tiles)
+            else:
+                out = self._tiled(z, False, tiles[:2], tiles[2:], frames=frames)
             return VAEOutput(sample=out.squeeze(2) if squeeze else out)
         assert z.shape[0] == 1 and z.shape[1] == 16
         _, _, T, h, w = z.shape
@@ -624,13 +657,20 @@ class B200VideoVAE(EngineModule):
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict=True, tiled=False, tile_size=None, tile_overlap=None, workspace=None):
         """x (1,3,T,H,W) or (1,3,H,W) in [-1,1] -> .latent (1,16,(T-1)/4+1,H/8,W/8) bf16 = posterior mode
-        (Encoder3D.forward + DiagonalGaussianDistribution.mode, attn_video_vae.py:1680-1689)."""
+        (Encoder3D.forward + DiagonalGaussianDistribution.mode, attn_video_vae.py:1680-1689).  ``tiled``: as in
+        ``decode`` (svr2_vae_encode_tiled; frames whose sides are not multiples of 8 run ``_tiled``)."""
         self._require_cuda("B200VideoVAE.encode")
         squeeze = x.ndim == 4
         if squeeze:
             x = x.unsqueeze(2)
         if tiled:
-            out = self._tiled(x, True, tile_size or (512, 512), tile_overlap or (64, 64))
+            tiles = tile_settings(tile_size or 512, 64 if tile_overlap is None else tile_overlap)
+            _, _, T, H, Wd = x.shape
+            if self._use_native() and H % 8 == 0 and Wd % 8 == 0:
+                out = torch.empty(1, 16, (T - 1) // 4 + 1, H // 8, Wd // 8, device=self.device, dtype=torch.bfloat16)
+                self._native_run(True, x[0].to(self.device).contiguous(), T, H, Wd, out, workspace, tiles=tiles)
+            else:
+                out = self._tiled(x, True, tiles[:2], tiles[2:])
             return VAEOutput(latent=out.squeeze(2) if squeeze else out, latent_dist=None)
         assert x.shape[0] == 1 and x.shape[1] == 3
         _, _, T, H, Wd = x.shape
@@ -682,18 +722,20 @@ class B200VideoVAE(EngineModule):
         return out
 
     # ---- spatial tiling (a25) ------------------------------------------------
-    def _tiled(self, src: torch.Tensor, encode: bool, tile_size, tile_overlap) -> torch.Tensor:
+    def _tiled(self, src: torch.Tensor, encode: bool, tile_size, tile_overlap, frames: Optional[int] = None) -> torch.Tensor:
         """VideoAutoencoderKL.tiled_encode / tiled_decode (attn_video_vae.py:1302-1630): the frame is cut into latent
         tiles of ``tile_size // 8`` stepping by ``tile - overlap // 8``; every tile runs through the whole (temporally
         sliced) encoder / decoder on its own and the results are cross-faded with raised-cosine ramps on interior
         edges — in latent space for encode, in sample space for decode — then normalised by the accumulated weights.
         Tiling changes results by design (tiles do not see their neighbours); it exists to bound memory.  The seam
-        arithmetic runs in bf16 with the reference's rounding points (``svr2_tile_accumulate_bf16``)."""
+        arithmetic runs in bf16 with the reference's rounding points (``svr2_tile_accumulate_bf16``).  ``frames``
+        (decode): each tile decodes only the first ``frames`` output frames.  The tile-by-tile sequencing in Python
+        (``.native = False``, profiling) of what svr2_vae_encode_tiled / svr2_vae_decode_tiled run natively."""
         dev = self.device
         _, _, _, H, W = src.shape
         f = 8
         th, tw = max(1, tile_size[0] // f), max(1, tile_size[1] // f)
-        run = (lambda t: self.encode(t).latent) if encode else (lambda t: self.decode(t).sample)
+        run = (lambda t: self.encode(t).latent) if encode else (lambda t: self.decode(t, frames=frames).sample)
         if (encode and H <= tile_size[0] and W <= tile_size[1]) or (not encode and H <= th and W <= tw):
             return run(src)
         loh, low = max(0, min(tile_overlap[0] // f, th - 1)), max(0, min(tile_overlap[1] // f, tw - 1))

@@ -150,7 +150,26 @@ int svr2_vae_decode(svr2_t* engine, const void* z, int z_dtype, int T, int h, in
 size_t svr2_vae_decode_frames_workspace_bytes(svr2_t* engine, int T, int h, int w, int slice_frames, int frames);
 int svr2_vae_decode_frames(svr2_t* engine, const void* z, int z_dtype, int T, int h, int w, int slice_frames, int frames,
                            void* sample, void* workspace, size_t workspace_bytes, void* stream);
-/* kernels launched by the handle's last svr2_vae_encode / svr2_vae_decode */
+/* Spatially tiled encode / decode (VideoAutoencoderKL.tiled_encode / tiled_decode, attn_video_vae.py:1302-1630): the frame
+ * is cut into latent tiles of tile / 8 pixels stepping by tile / 8 - overlap / 8 (overlap clamped below the tile), tiles
+ * wholly inside the previous one's overlap skipped; every tile runs the whole encoder / decoder (temporal slices of
+ * `slice_frames`, its own slicing state) on its window of the input, and its final kernel accumulates it into the result
+ * with raised-cosine edge weights (svr2_conv_tap_gather_seam_bf16 / svr2_ndhwc_to_ncdhw_seam_bf16), then the result is
+ * normalised by the summed weights.  Ramps over `overlap` sample pixels for decode, overlap / 8 latent pixels for encode.
+ * The same tiles, order and bf16 rounding points as the tile-by-tile sequence with svr2_tile_accumulate_bf16.  A frame
+ * that fits one tile (encode: H <= tile_h and W <= tile_w; decode: h <= tile_h / 8 and w <= tile_w / 8) runs un-tiled.
+ * Shapes, dtypes and `frames` as svr2_vae_encode / svr2_vae_decode_frames; tile sizes >= 1 and overlaps >= 0 in sample
+ * pixels.  Everything, the count plane included, lives in the one workspace; the query (direction 0 encode, 1 decode;
+ * `frames` ignored by an encode) is exact and a smaller workspace is refused. */
+size_t svr2_vae_tiled_workspace_bytes(svr2_t* engine, int direction, int T, int H, int W, int tile_h, int tile_w,
+                                      int overlap_h, int overlap_w, int slice_frames, int frames);
+int svr2_vae_encode_tiled(svr2_t* engine, const void* x, int x_dtype, int T, int H, int W, int tile_h, int tile_w,
+                          int overlap_h, int overlap_w, int slice_frames, void* latent, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int svr2_vae_decode_tiled(svr2_t* engine, const void* z, int z_dtype, int T, int h, int w, int tile_h, int tile_w,
+                          int overlap_h, int overlap_w, int slice_frames, int frames, void* sample, void* workspace,
+                          size_t workspace_bytes, void* stream);
+/* kernels launched by the handle's last svr2_vae_encode / svr2_vae_decode (tiled ones included) */
 int64_t svr2_vae_last_launches(svr2_t* engine);
 
 /* ---- K1: Linear.  out[M,N] = epi(a[M,K] @ w[N,K]^T).  Replaces nn.Linear at
@@ -370,6 +389,29 @@ int svr2_tile_accumulate_bf16(const void* tile, int64_t tile_plane_stride, int t
                               int eff_w, const void* weight_h, const void* weight_w, void* result, void* count, int H,
                               int W, int y0, int x0, void* stream);
 int svr2_tile_normalize_bf16(void* result, const void* count, int planes, int64_t hw, void* stream);
+/* The raised-cosine ramps of the seams, computed in torch's CUDA bf16 arithmetic (each op rounded to bf16):
+ * r = 0.5 - 0.5 * cos(linspace(0, 1, n) * pi) with linspace's two-sided formula (step = 1 / (n - 1); the first n / 2
+ * entries step * i, the rest 1 - step * (n - 1 - i)).  ramp [2n] = [r | 1 - r]; one launch for both tables of a clip
+ * (len 0: that table is not written). */
+int svr2_tile_ramp_bf16(void* ramp_h, int len_h, void* ramp_w, int len_w, void* stream);
+/* Seam variants of the tiled passes' final kernels: instead of storing the tile, accumulate it into the clip-sized
+ * result as svr2_tile_accumulate_bf16 does with the stored tile (bit-identical).  result / count point at the tile's
+ * top-left corner (count: row stride row_stride; NULL leaves it alone — later temporal slices of a tile), strides in
+ * elements.  Edge weights per axis of n tile pixels: ones; with a neighbour before (SVR2_SEAM_TOP / LEFT) the first
+ * ov = min(len, n - 1) entries r[i]; with one after (BOTTOM / RIGHT) the last ov entries (1 - r)[i], which win where
+ * both apply.
+ *   conv_tap_gather: the tile is bf16(bias + sum over the 27 taps), as svr2_conv_tap_gather writes it (co_n <= 4);
+ *   ndhwc_to_ncdhw:  the tile is the first C (<= 16) channels of in [T, H, W, ld_in]. */
+#define SVR2_SEAM_TOP 1
+#define SVR2_SEAM_BOTTOM 2
+#define SVR2_SEAM_LEFT 4
+#define SVR2_SEAM_RIGHT 8
+int svr2_conv_tap_gather_seam_bf16(const float* z, int64_t ldz, int co_n, const void* bias, int T, int H, int W,
+                                   void* result, int64_t chan_stride, int64_t frame_stride, int row_stride, void* count,
+                                   const void* ramp_h, int len_h, const void* ramp_w, int len_w, int edges, void* stream);
+int svr2_ndhwc_to_ncdhw_seam_bf16(const void* in, int ld_in, int C, int T, int H, int W, void* result, int64_t chan_stride,
+                                  int64_t frame_stride, int row_stride, void* count, const void* ramp_h, int len_h,
+                                  const void* ramp_w, int len_w, int edges, void* stream);
 
 /* ---- Clip pre-processing (prepare_video_transforms, src/core/generation_utils.py:72-84; SURVEY.md §8(f) rank 3).
  * Antialiased bicubic resize (torchvision resize -> torch _upsample_bicubic2d_aa semantics, fp32 accumulation, result
