@@ -8,7 +8,8 @@
 // temporal halo is two real frames stored in front of every activation tensor).
 //
 // Roles (384 threads, 1 CTA / SM, grid = #SMs, static tile schedule):
-//   warps 0,3  : TMA producers (even / odd k-blocks of a kStages-deep smem ring, 128B-swizzled K-major tiles)
+//   warps 0,3  : TMA producers (even / odd k-blocks of a kStages-deep smem ring, 128B-swizzled K-major tiles;
+//                SLAB convs: warp 0 a weight ring, warp 3 a ring of activation slabs, see SlabLayout)
 //   warps 4-11 : two MMA warpgroups (wgmma m64 x BLOCK_N x 16, 64 tile rows each, fp32 accumulators in registers)
 //   KIND_BF16  : the MMA warpgroups round bf16(acc + bias) into a dedicated bf16 tile and go on with the next tile's
 //                MMAs; warps 1,2 run the rest of the epilogue from that tile (activation, gate, residual, GroupNorm
@@ -121,6 +122,27 @@ struct SmemLayout {
   static constexpr int kStagingOffset = kStages * kStageBytes;
   static constexpr int kBarOffset = kStagingOffset + kStagingBytes;
   static constexpr int kTotal = kBarOffset + 256 + 1024;  // barriers + alignment slack
+};
+
+// Slab mainloop (SLAB: stride-1 3x3 convs on the swap-AB and the 256-column tiles).  The taps kh = 0, 1, 2 of one
+// (kt, kw, channel block) read the same bw x bh activation box shifted down by one image row each, so one bw x (bh + 2)
+// box -- the slab -- holds all three: tap kh is the slab from row kh on, kh * bw * 128 bytes in, a whole number of
+// 1024-byte swizzle atoms for every tile shape that takes this path.  The ring splits in two: a weight ring of one
+// k-block's weight tile per stage and a slab ring of one slab per stage, both sized from SmemLayout's budget.  (The
+// one-ring members it inherits only let the ring code, which a SLAB kernel never runs, compile.)
+template <bool SWAP>
+struct SlabLayout : SmemLayout<256, true> {
+  using Base = SmemLayout<256, true>;
+  static constexpr int kWBytes = (SWAP ? BLOCK_M : 256) * BLOCK_K * 2;          // 16 KB / 32 KB
+  static constexpr int kSBytes = (SWAP ? 32 * 10 : 16 * 10) * BLOCK_K * 2;      // the widest slab: 32 x 10 / 16 x 10 px
+  static constexpr int kSStages = SWAP ? 2 : 3;
+  static constexpr int kWStages = (Base::kBudget - kSStages * kSBytes) / kWBytes;
+  static constexpr int kStages = kWStages + kSStages;   // barriers: the weight stages, then the slab stages
+  static constexpr int kSlabOffset = kWStages * kWBytes;
+  static constexpr int kStagingOffset = kSlabOffset + kSStages * kSBytes;
+  static constexpr int kBarOffset = kStagingOffset + Base::kStagingBytes;
+  static constexpr int kTotal = kBarOffset + 256 + 1024;
+  static_assert(kWStages >= 3 && kSBytes % 1024 == 0 && kTotal <= 232448, "slab rings do not fit");
 };
 
 // 32 consecutive fp32 accumulator columns of one row of the shared accumulator tile (idx: element offset, % 4 == 0)
@@ -266,14 +288,17 @@ __device__ __forceinline__ RowDest row_dest(const GemmParams& p, int epi, int m_
 // EPI_CT >= 0: the epilogue flags are a compile-time constant (p.epi must equal it) — the per-element loops then carry
 // no runtime flag tests.  A single such test cost the short-K pixel-shuffle GEMM 50 % (its epilogue, ~1 800 warp
 // instructions per tile, is the whole kernel); EPI_CT = -1 keeps the generic runtime-flag epilogue.
-template <int BLOCK_N, int KIND, bool SWAP = false, int EPI_CT = -1>
+// SLAB: the slab mainloop (SlabLayout); tmap_a then has the box (64, bw, bh + 2, 1).
+template <int BLOCK_N, int KIND, bool SWAP = false, int EPI_CT = -1, bool SLAB = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_a2, const GemmParams p) {
   if (p.run_if != nullptr && *p.run_if == 0) return;     // conditional launch: every thread of every CTA sees the same flag
   constexpr bool EPI_WG = kEpiWG<KIND>;
   static_assert(EPI_WG || (!SWAP && EPI_CT < 0), "swap-AB and compile-time epilogues are KIND_BF16 only");
-  using L = SmemLayout<BLOCK_N, EPI_WG>;
+  static_assert(!SLAB || (KIND == KIND_BF16 && BLOCK_N == 256), "the slab mainloop is KIND_BF16 with 256-column tiles");
+  using S = SlabLayout<SWAP>;
+  using L = std::conditional_t<SLAB, S, SmemLayout<BLOCK_N, EPI_WG>>;
   constexpr int kStages = L::kStages;
   constexpr int ACC_STRIDE = BLOCK_N < 32 ? 32 : BLOCK_N;   // accumulator columns the epilogue addresses
   constexpr int ACC_LD = ACC_STRIDE + 4;                    // fp32 row pitch of the shared accumulator tile
@@ -319,11 +344,74 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   if (warp == 0 || warp == 3) {
     // ========================= TMA producers (2 warps) =========================
-    // One thread of warp 0 feeds the even k-blocks of the ring, one thread of warp 3 the odd ones, so that the
-    // per-k-block issue path (barrier poll, expect-tx, two TMA issues) of one thread never paces the MMAs.
-    // Without the epilogue warps the shared accumulator tile of the epilogue overlays the ring: a tile's loads
-    // start once the previous tile's epilogue has released it (acc_free).
-    if (lane == 0) {
+    if constexpr (SLAB) {
+      // One thread of warp 0 feeds the weight ring (one stage per k-block), one thread of warp 3 the slab ring (one
+      // stage per (kt, kw, channel block), then one per shortcut k-block, holding its bw x bh box).  A tile's k-blocks
+      // run kt, kw, channel block, kh = 0, 1, 2; the weight column of a tap is ((kt 3 + kh) 3 + kw) Cin + 64 cb.
+      if (lane == 0) {
+        const bool wgt = warp == 0;
+        const int n_st = wgt ? S::kWStages : S::kSStages;
+        const int bar0 = wgt ? 0 : S::kWStages;
+        const int st_bytes = wgt ? S::kWBytes : S::kSBytes;
+        uint8_t* const ring = smem + (wgt ? 0 : S::kSlabOffset);
+        int stage = 0;
+        uint32_t phase = 0;
+        auto acquire = [&](uint32_t bytes, uint64_t*& fb) -> uint8_t* {
+          mbar_wait(&empty_bar[bar0 + stage], phase ^ 1);
+          fb = &full_bar[bar0 + stage];
+          mbar_expect_tx(fb, bytes);
+          uint8_t* s = ring + stage * st_bytes;
+          if (++stage == n_st) { stage = 0; phase ^= 1; }
+          return s;
+        };
+        const int bw = p.bw, bh = p.bh, taps_t = p.taps_t, cin_blocks = p.cin_blocks, cin = p.cin;
+        const uint32_t slab_bytes = bw * (bh + 2) * BLOCK_K * 2, box_bytes = bw * bh * BLOCK_K * 2;
+        for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+          int m_blk, n_blk, t_o, th, tw;
+          tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
+          conv_tile(p, m_blk, t_o, th, tw);
+          const int h0 = th * bh, w0 = tw * bw;
+          int n0 = n_blk * (SWAP ? BLOCK_M : BLOCK_N);
+          int taps = taps_t, kcol = 0;
+          if (t_o < p.fold_t) {      // folded head, as in the ring producer below
+            taps = t_o + 1;
+            kcol = t_o == 0 ? 2 * 9 * cin : 0;
+            n0 += p.fold_n;
+          }
+          uint64_t* fb;
+          for (int kt_ = 0; kt_ < taps; ++kt_) {
+            const int t_in = t_o * p.stride_t + taps_t - taps + kt_;
+            for (int kw_ = 0; kw_ < 3; ++kw_) {
+              for (int cb = 0; cb < cin_blocks; ++cb) {
+                if (wgt) {
+                  for (int kh_ = 0; kh_ < 3; ++kh_) {
+                    uint8_t* s = acquire(S::kWBytes, fb);
+                    tma_load_2d(s, &tmap_b, fb, kcol + ((kt_ * 3 + kh_) * 3 + kw_) * cin + cb * BLOCK_K, n0);
+                  }
+                } else {
+                  uint8_t* s = acquire(slab_bytes, fb);
+                  tma_load_4d(s, &tmap_a, fb, cb * BLOCK_K, w0 + kw_ - p.pad_w, h0 - p.pad_h, t_in);
+                }
+              }
+            }
+          }
+          kcol += taps * 9 * cin;
+          for (int cb = 0; cb < p.extra_blocks; ++cb) {
+            if (wgt) {
+              uint8_t* s = acquire(S::kWBytes, fb);
+              tma_load_2d(s, &tmap_b, fb, kcol + cb * BLOCK_K, n0);
+            } else {
+              uint8_t* s = acquire(box_bytes, fb);
+              tma_load_4d(s, &tmap_a2, fb, cb * BLOCK_K, w0, h0, t_o);
+            }
+          }
+        }
+      }
+    } else if (lane == 0) {
+      // One thread of warp 0 feeds the even k-blocks of the ring, one thread of warp 3 the odd ones, so that the
+      // per-k-block issue path (barrier poll, expect-tx, two TMA issues) of one thread never paces the MMAs.
+      // Without the epilogue warps the shared accumulator tile of the epilogue overlays the ring: a tile's loads
+      // start once the previous tile's epilogue has released it (acc_free).
       int stage = 0;
       uint32_t phase = 0;
       uint32_t g = (warp == 0) ? 0u : 1u;   // parity toggle: handle a k-block when (g & 1) == 0
@@ -457,6 +545,58 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
       tail(d);
     };
+    // Slab mainloop: k-block kb waits on its weight stage and, at the first k-block of a slab, on the slab stage, and
+    // reads the slab from row kh on.  A stage is released once the MMAs of the last k-block that reads it have retired
+    // (the same one-group-in-flight rule, per ring).  The shortcut's k-blocks are one-use slabs read from row 0.
+    int wstage = 0, sstage = 0;
+    uint32_t wphase = 0, sphase = 0;
+    auto mainloop_slab = [&](int nkb, auto&& tail) {
+      float d[BLOCK_N / 2];
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
+      const bool leader = (threadIdx.x & 127) == 0;
+      const int nkb_taps = nkb - p.extra_blocks;            // a multiple of 3: slabs of kh = 0, 1, 2
+      const uint32_t row_bytes = p.bw * BLOCK_K * 2;
+      const uint32_t w_ring = smem_u32(smem), s_ring = smem_u32(smem + S::kSlabOffset);
+      int prev_w = -1, prev_s = -1, kh = 0;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full_bar[wstage], wphase);
+        if (kh == 0) mbar_wait(&full_bar[S::kWStages + sstage], sphase);
+        const uint32_t w_addr = w_ring + wstage * S::kWBytes;
+        const uint32_t s_addr = s_ring + sstage * S::kSBytes + kh * row_bytes;
+        const uint64_t a_desc = wgmma_desc_kmajor_sw128((SWAP ? w_addr : s_addr) + wg * 64 * 128);
+        const uint64_t b_desc = wgmma_desc_kmajor_sw128(SWAP ? s_addr : w_addr);
+        wgmma_fence_regs(d);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
+          wgmma_ss<BLOCK_N>(d, a_desc + uint64_t(k * 2), b_desc + uint64_t(k * 2), (kb | k) != 0);
+        wgmma_commit();
+        wgmma_fence_regs(d);
+        wgmma_wait<1>();
+        if (leader) {
+          if (prev_w >= 0) mbar_arrive(&empty_bar[prev_w]);
+          if (prev_s >= 0) mbar_arrive(&empty_bar[S::kWStages + prev_s]);
+        }
+        prev_w = wstage;
+        if (++wstage == S::kWStages) { wstage = 0; wphase ^= 1; }
+        prev_s = -1;
+        if (kh == 2 || kb >= nkb_taps) {                    // the last k-block that reads this slab
+          prev_s = sstage;
+          if (++sstage == S::kSStages) { sstage = 0; sphase ^= 1; }
+          kh = 0;
+        } else {
+          ++kh;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      if (leader) {
+        if (prev_w >= 0) mbar_arrive(&empty_bar[prev_w]);
+        if (prev_s >= 0) mbar_arrive(&empty_bar[S::kWStages + prev_s]);
+      }
+      tail(d);
+    };
     const int epi = EPI_CT >= 0 ? EPI_CT : p.epi;
     const __nv_bfloat16* __restrict__ bias = p.bias;
     if constexpr (EPI_WG) {
@@ -514,7 +654,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       for (int tile = tile0; tile < num_tiles; tile += tile_step, ++it) {
         int m_blk, n_blk;
         tile_coords(tile, num_m_tiles, num_n_tiles, p.group_n, m_blk, n_blk);
-        mainloop(conv_k_blocks(p, m_blk), [&](float (&d)[BLOCK_N / 2]) { store_tile(d, n_blk); });
+        auto store = [&](float (&d)[BLOCK_N / 2]) { store_tile(d, n_blk); };
+        if constexpr (SLAB) mainloop_slab(conv_k_blocks(p, m_blk), store);
+        else mainloop(conv_k_blocks(p, m_blk), store);
       }
     } else {
       // The accumulators go to a row-major fp32 tile in shared memory (over the drained operand ring), and the
@@ -1134,12 +1276,12 @@ int num_sms() {
   return g_num_sms[dev];
 }
 
-template <int BLOCK_N, int KIND, bool SWAP = false, int EPI_CT = -1>
+template <int BLOCK_N, int KIND, bool SWAP = false, int EPI_CT = -1, bool SLAB = false>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p_in, cudaStream_t stream,
                        const CUtensorMap* ta2_opt = nullptr) {
   const CUtensorMap& ta2 = ta2_opt ? *ta2_opt : ta;
-  using L = SmemLayout<BLOCK_N, kEpiWG<KIND>>;
-  auto kern = gemm_wgmma_kernel<BLOCK_N, KIND, SWAP, EPI_CT>;
+  using L = std::conditional_t<SLAB, SlabLayout<SWAP>, SmemLayout<BLOCK_N, kEpiWG<KIND>>>;
+  auto kern = gemm_wgmma_kernel<BLOCK_N, KIND, SWAP, EPI_CT, SLAB>;
   GemmParams p = p_in;
   {
     // raster group: keep the group's B slice around 16 MB (L2 = 50 MB, shared with A tiles and the output stream)
@@ -1424,6 +1566,19 @@ static void conv_tile_shape(int Cout, int H_out, int W_out, bool* swap_out, int*
   }
   *swap_out = swap; *bw_out = bw; *bh_out = bh;
 }
+// The slab mainloop (SlabLayout) serves stride-1 convs with 3x3 spatial taps and a temporal kernel on the swap-AB tiles
+// and on the 256-column tiles of two or more tile rows; every other conv runs the one-ring mainloop.
+static bool conv_slab(int Cout, int kt, int kh, int kw, int stride_hw, int H_out, int W_out) {
+  bool swap;
+  int bw, bh;
+  conv_tile_shape(Cout, H_out, W_out, &swap, &bw, &bh);
+  return stride_hw == 1 && kt > 1 && kh == 3 && kw == 3 && bh > 1 && (swap || pick_block_n(Cout, 0) == 256);
+}
+extern "C" int svr2_conv_mainloop(int Cin, int Cout, int kt, int kh, int kw, int stride_hw, int H, int W) {
+  if (Cin <= 0 || Cin % 64 || Cout <= 0 || (stride_hw != 1 && stride_hw != 2))
+    return set_error(SVR2_ERR_ARG, "svr2_conv_mainloop: Cin must be a positive multiple of 64, stride_hw 1 or 2");
+  return conv_slab(Cout, kt, kh, kw, stride_hw, stride_hw == 1 ? H : H / 2, stride_hw == 1 ? W : W / 2) ? 1 : 0;
+}
 // GroupNorm partial-sum slots per frame a conv with statistics writes (the size query of svr2_conv3d_stats_bf16 without
 // the tensor maps: workspace planning)
 extern "C" int svr2_conv_stat_slots(int Cout, int H_out, int W_out) {
@@ -1447,12 +1602,13 @@ static int conv3d_impl(const void* x, int T_in_total, int H, int W, int Cin, con
   int bw, bh;
   conv_tile_shape(Cout, H_out, W_out, &swap, &bw, &bh);
   const int bn = swap ? 128 : pick_block_n(Cout, 0);
+  const bool slab = conv_slab(Cout, kt, kh, kw, stride_hw, H_out, W_out);
   CUtensorMap ta, tb;
   int rc;
   if (stride_hw == 1) {
     uint64_t d[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)T_in_total};
     uint64_t s[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-    uint32_t b[4] = {BLOCK_K, (uint32_t)bw, (uint32_t)bh, 1};
+    uint32_t b[4] = {BLOCK_K, (uint32_t)bw, (uint32_t)(slab ? bh + 2 : bh), 1};
     rc = make_tmap_bf16(&ta, x, 4, d, s, b);
   } else {
     uint64_t d[5] = {(uint64_t)Cin * 2, (uint64_t)W / 2, 2, (uint64_t)H / 2, (uint64_t)T_in_total};
@@ -1527,6 +1683,13 @@ static int conv3d_impl(const void* x, int T_in_total, int H, int W, int Cin, con
     if (stat_bytes < need) return set_error(SVR2_ERR_ARG, "conv stats: stat_partial buffer too small");
     p.stat_partial = (float4*)stat_partial;
     p.stat_slots = slots;
+  }
+  const CUtensorMap* ta2p = x2 ? &ta2 : nullptr;
+  if (slab) {
+    if (swap) return launch_gemm<256, KIND_BF16, true, -1, true>(ta, tb, p, (cudaStream_t)stream, ta2p);
+    if (p.epi == EPI_BIAS && !x2)
+      return launch_gemm<256, KIND_BF16, false, EPI_BIAS, true>(ta, tb, p, (cudaStream_t)stream);
+    return launch_gemm<256, KIND_BF16, false, -1, true>(ta, tb, p, (cudaStream_t)stream, ta2p);
   }
   if (swap) return launch_gemm<256, KIND_BF16, true>(ta, tb, p, (cudaStream_t)stream, x2 ? &ta2 : nullptr);
   return dispatch_gemm(bn, ta, tb, p, (cudaStream_t)stream, x2 ? &ta2 : nullptr);

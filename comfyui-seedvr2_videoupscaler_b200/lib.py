@@ -12,7 +12,8 @@ from ctypes import c_float, c_int, c_int64, c_void_p, POINTER
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("SVR2_LIB") or os.path.join(HERE, "csrc", "libsvr2.so")   # SVR2_LIB: another build (A/B tools only)
+DEFAULT_LIB_PATH = os.path.join(HERE, "csrc", "libsvr2.so")
+LIB_PATH = os.environ.get("SVR2_LIB") or DEFAULT_LIB_PATH   # SVR2_LIB: another build (A/B tools only)
 
 EPI_BIAS, EPI_GATE, EPI_RESIDUAL, EPI_SWIGLU, EPI_GELU, EPI_F32, EPI_SILU = 1, 2, 4, 8, 16, 32, 128
 EPI_ROWSTAT, EPI_PEXP, EPI_ROWSCALE, EPI_FOLD_HEAD = 256, 512, 1024, 2048
@@ -67,6 +68,7 @@ SIGNATURES = {
     "svr2_conv3d_shortcut_stats_bf16": [_P, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int,
                                         _P, c_int, c_int, _P, c_int64, POINTER(c_int), _P],
     "svr2_conv_stat_slots": [c_int, c_int, c_int],
+    "svr2_conv_mainloop": [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int],
     "svr2_groupnorm_from_stats_bf16": [_P, _P, c_int, c_int, c_int, _P, _P, c_float, c_int, c_int, c_int, _P, c_int, _P,
                                        _P],
     "svr2_upsample_shuffle_bf16": [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int, c_int, _P],
@@ -147,6 +149,9 @@ def load() -> ctypes.CDLL:
         lib.svr2_engine_last_error.restype = ctypes.c_char_p
         lib.svr2_engine_last_error.argtypes = [c_void_p]
         for name, args in SIGNATURES.items():
+            fn = getattr(lib, name, None)
+            if fn is None and LIB_PATH != DEFAULT_LIB_PATH:
+                continue      # an older build loaded for an A/B timing: calling an entry point it lacks fails there
             fn = getattr(lib, name)
             fn.restype = c_int64 if (name.endswith("_bytes") or name == "svr2_vae_last_launches") else (None if name == "svr2_destroy" else c_int)
             fn.argtypes = args

@@ -206,6 +206,12 @@ int svr2_conv3d_stats_bf16(const void* x, int T_in_total, int H, int W, int Cin,
  * lets a caller plan memory without the NULL query) */
 int svr2_conv_stat_slots(int Cout, int H_out, int W_out);
 
+/* which mainloop svr2_conv3d_bf16 runs for a geometry (H, W: the input's; a pure function of the arguments): 0 the
+ * one-ring mainloop, 1 the slab mainloop, in which one activation box of bh + 2 rows feeds the three vertical taps kh of
+ * each (kt, kw, 64-channel block) -- stride-1 convs with kh = kw = 3 and kt > 1 on the swap-AB tiles (64 < Cout <= 128)
+ * and on the 256-column tiles (Cout >= 256) of 16 x 8 / 8 x 16 pixels.  Negative: invalid Cin or stride_hw. */
+int svr2_conv_mainloop(int Cin, int Cout, int kt, int kh, int kw, int stride_hw, int H, int W);
+
 /* Stride-1 causal conv with the ResnetBlock3D 1x1x1 conv_shortcut fused in as extra K-blocks (attn_video_vae.py:311-362:
  * `x = conv_shortcut(x); return x + hidden`): y = conv(x; w[:, :kt*kh*kw*Cin]) + x2 . w[:, kt*kh*kw*Cin:]^T + bias,
  * x2 = [T_out, H, W, C2] bf16 (the block input, no halo, C2 % 64 == 0), w = [Cout][kt*kh*kw*Cin + C2] (conv2 weight rows
