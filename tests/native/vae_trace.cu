@@ -1,8 +1,18 @@
 // Test harness (CPU): the native VAE runtime (csrc/vae_engine.cu) compiled with SVR2_HOST_TEST — host memory as the
 // workspace, every kernel entry point replaced by a stub that prints its name and scalar arguments (pointers as p0 / p1
-// = NULL / not NULL).  tests/test_native_vae_cpu.py compares the trace with the op sequence of the Python module
-// (vae.py) on the same clip, and the dry-run workspace size with the extent the real run touches.
-// usage: vae_trace <weights manifest> enc|dec T H W slice_frames
+// = NULL / not NULL).  The tests compare the trace with the op sequence of the Python module (vae.py) on the same clip,
+// and the dry-run workspace size with the extent the real run touches.
+// usage: vae_trace fuzz
+//        vae_trace <weights manifest> enc|dec T H W slice_frames                  svr2_vae_encode / svr2_vae_decode
+//        vae_trace <weights manifest> frames T h w slice_frames frames [plan]     svr2_vae_decode_frames
+//        vae_trace <weights manifest> tiled enc|dec T H W tile_h tile_w overlap_h overlap_w slice_frames frames [plan]
+//                                                                                 svr2_vae_encode_tiled / _decode_tiled
+//   A pass prints the trace, then "# workspace <bytes> touched_max_offset <bytes> launches <n>" ("plan": only
+//   "# workspace <bytes>").  A refused plan exits 3: "plan failed: <message>" on stderr for enc|dec, "refused: <message>"
+//   for tiled, and for frames "refused: <query's message> | <decode's message>" when the decode refuses as well.
+//   A seam line ends with "| <offset of the tile's corner in the result, elements> <channel stride> <frame stride>
+//   <row stride> <count p0/p1> <ramp lengths> <edges>"; a windowed conversion with "| <channel, frame, row strides>
+//   <offset of the window in the input, elements>".
 #define SVR2_HOST_TEST 1
 #include "../../comfyui-seedvr2_videoupscaler_b200/csrc/vae_engine.cu"
 #include <stdarg.h>
@@ -18,6 +28,8 @@ int set_error(int code, const char* m) { snprintf(g_msg, sizeof g_msg, "%s", m ?
 static char* g_lo = nullptr;
 static char* g_hi = nullptr;       // workspace bounds: every non-NULL pointer into it must stay inside
 static size_t g_touch = 0;
+static const char* g_in = nullptr;  // a tiled pass's input and result (bf16): windows and seams print offsets into them
+static const char* g_out = nullptr;
 static const char* P_(const void* p) {
   if (p && (const char*)p >= g_lo && (const char*)p < g_hi) {
     const size_t off = (const char*)p - g_lo;
@@ -131,7 +143,38 @@ int conv_tap_gather_strided(const float* z, int64_t ldz, int co_n, const void* b
          P_(stream), (long long)cs);
   return 0;
 }
+// the tiled passes' own launches: the windowed input conversion, the seam variants of the final kernels, the ramp tables
+int ncdhw_to_ndhwc_window(const void* in, int in_dtype, int C, int T, int H, int W, int64_t cs, int64_t fs, int rs, void* out,
+                          int C_pad, int out_t_pad, float div, void* stream) {
+  printf("svr2_ncdhw_to_ndhwc_window %s %d %d %d %d %d %s %d %d %.5g %s | %lld %lld %d %lld\n", P_(in), in_dtype, C, T, H, W, P_(out),
+         C_pad, out_t_pad, div, P_(stream), (long long)cs, (long long)fs, rs, (long long)(((const char*)in - g_in) / 2));
+  return 0;
+}
+static void seam_suffix(const Seam& s) {
+  printf(" | %lld %lld %lld %d %s %d %d %d\n", (long long)(((const char*)s.result - g_out) / 2), (long long)s.cs, (long long)s.fs,
+         s.rs, P_(s.count), s.len_h, s.len_w, s.edges);
+  P_(s.ramp_h);
+  P_(s.ramp_w);
+}
+int conv_tap_gather_seam(const float* z, int64_t ldz, int co_n, const void* bias, int T, int H, int W, const Seam& s, void* stream) {
+  printf("svr2_conv_tap_gather_seam %s %lld %d %s %d %d %d %s", P_(z), (long long)ldz, co_n, P_(bias), T, H, W, P_(stream));
+  seam_suffix(s);
+  return 0;
+}
+int ndhwc_to_ncdhw_seam(const void* in, int ld_in, int C, int T, int H, int W, const Seam& s, void* stream) {
+  printf("svr2_ndhwc_to_ncdhw_seam %s %d %d %d %d %d %s", P_(in), ld_in, C, T, H, W, P_(stream));
+  seam_suffix(s);
+  return 0;
+}
+int tile_ramp(void* ramp_h, int len_h, void* ramp_w, int len_w, void* stream) {
+  printf("svr2_tile_ramp_bf16 %s %d %s %d %s\n", P_(ramp_h), len_h, P_(ramp_w), len_w, P_(stream));
+  return 0;
+}
 }  // namespace svr2
+extern "C" int svr2_tile_normalize_bf16(void* result, const void* count, int planes, int64_t hw, void* stream) {
+  printf("svr2_tile_normalize_bf16 %s %s %d %lld %s\n", result ? "p1" : "p0", P_(count), planes, (long long)hw, P_(stream));
+  return 0;
+}
 
 // Arena fuzz: a random alloc / release / alloc_top sequence replayed on an unbounded arena (the dry run) and on one capped
 // at the dry run's need() must make identical placement decisions, never overlap two live blocks and stay inside the cap.
@@ -185,6 +228,30 @@ static int arena_fuzz(unsigned seed, int ops) {
   return 0;
 }
 
+// One traced pass: given its exact plan `need`, prints only that ("plan"), or runs the pass in a host workspace of that size
+// with a result of `out_bytes`, checks that a workspace 256 bytes short is refused and prints the summary line.
+// pass(ws, ws_bytes, out) calls the entry point under test.
+template <class Pass>
+static int trace(svr2_engine& eng, size_t need, bool plan_only, size_t out_bytes, Pass pass) {
+  if (plan_only) {
+    printf("# workspace %zu\n", need);
+    return 0;
+  }
+  std::vector<char> out(out_bytes);
+  g_out = out.data();
+  void* ws = nullptr;
+  if (posix_memalign(&ws, 256, need)) return 4;
+  g_lo = (char*)ws;
+  g_hi = g_lo + need;
+  if (const int rc = pass(ws, need, out.data())) { fprintf(stderr, "run failed (%d): %s\n", rc, eng.err); return 5; }
+  const int64_t launches = svr2_vae_last_launches(&eng);
+  if (pass(ws, need - 256, out.data()) == 0) return 6;
+  printf("# workspace %zu touched_max_offset %zu launches %lld\n", need, g_touch, (long long)launches);
+  free(ws);
+  vae_state_destroy(&eng);
+  return 0;
+}
+
 int main(int argc, char** argv) {
   if (argc >= 2 && std::string(argv[1]) == "fuzz") {
     for (unsigned seed = 1; seed <= 200; ++seed) {
@@ -208,23 +275,48 @@ int main(int argc, char** argv) {
     t.ptr = (void*)0x1000;
     eng.w[name] = t;
   }
-  const bool enc = std::string(argv[2]) == "enc";
-  const int T = atoi(argv[3]), H = atoi(argv[4]), W = atoi(argv[5]), slice = atoi(argv[6]);
-  const size_t need = svr2_vae_workspace_bytes(&eng, enc ? 0 : 1, T, H, W, slice);
-  if (!need) { fprintf(stderr, "plan failed: %s\n", eng.err); return 3; }
-  void* ws = nullptr;
-  if (posix_memalign(&ws, 256, need)) return 4;
-  g_lo = (char*)ws;
-  g_hi = g_lo + need;
-  static char in_buf[16], out_buf[16];
-  const int rc = enc ? svr2_vae_encode(&eng, in_buf, 1, T, H, W, slice, out_buf, ws, need, nullptr)
-                     : svr2_vae_decode(&eng, in_buf, 1, T, H, W, slice, out_buf, ws, need, nullptr);
-  if (rc) { fprintf(stderr, "run failed (%d): %s\n", rc, eng.err); return 5; }
-  // a workspace one byte short of the plan must be refused
-  if ((enc ? svr2_vae_encode(&eng, in_buf, 1, T, H, W, slice, out_buf, ws, need - 256, nullptr)
-           : svr2_vae_decode(&eng, in_buf, 1, T, H, W, slice, out_buf, ws, need - 256, nullptr)) == 0) return 6;
-  printf("# workspace %zu touched_max_offset %zu launches %lld\n", need, g_touch, (long long)svr2_vae_last_launches(&eng));
-  free(ws);
-  vae_state_destroy(&eng);
-  return 0;
+  const std::string mode = argv[2];
+  auto arg = [&](int i) { return atoi(argv[i]); };
+  auto plan_only = [&](int i) { return argc > i && std::string(argv[i]) == "plan"; };
+  static char in[16];
+  g_in = in;
+  if (mode == "enc" || mode == "dec") {
+    const bool enc = mode == "enc";
+    const int T = arg(3), H = arg(4), W = arg(5), slice = arg(6);
+    const size_t need = svr2_vae_workspace_bytes(&eng, enc ? 0 : 1, T, H, W, slice);
+    if (!need) { fprintf(stderr, "plan failed: %s\n", eng.err); return 3; }
+    return trace(eng, need, false, 16, [&](void* ws, size_t bytes, void* out) {
+      return enc ? svr2_vae_encode(&eng, in, 1, T, H, W, slice, out, ws, bytes, nullptr)
+                 : svr2_vae_decode(&eng, in, 1, T, H, W, slice, out, ws, bytes, nullptr);
+    });
+  }
+  if (mode == "frames" && argc >= 8) {
+    const int T = arg(3), h = arg(4), w = arg(5), slice = arg(6), frames = arg(7);
+    const size_t need = svr2_vae_decode_frames_workspace_bytes(&eng, T, h, w, slice, frames);
+    if (!need) {        // the decode itself must refuse `frames` too
+      const std::string msg = eng.err;
+      static char small_ws[1 << 12] __attribute__((aligned(256)));
+      static char out[16];
+      if (svr2_vae_decode_frames(&eng, in, 1, T, h, w, slice, frames, out, small_ws, sizeof small_ws, nullptr) == 0) return 8;
+      fprintf(stderr, "refused: %s | %s\n", msg.c_str(), eng.err);
+      return 3;
+    }
+    return trace(eng, need, plan_only(8), 16, [&](void* ws, size_t bytes, void* out) {
+      return svr2_vae_decode_frames(&eng, in, 1, T, h, w, slice, frames, out, ws, bytes, nullptr);
+    });
+  }
+  if (mode == "tiled" && argc >= 13) {
+    const bool enc = std::string(argv[3]) == "enc";
+    const int T = arg(4), H = arg(5), W = arg(6), th = arg(7), tw = arg(8), oh = arg(9), ow = arg(10), slice = arg(11),
+              frames = arg(12);
+    const size_t need = svr2_vae_tiled_workspace_bytes(&eng, enc ? 0 : 1, T, H, W, th, tw, oh, ow, slice, frames);
+    if (!need) { fprintf(stderr, "refused: %s\n", eng.err); return 3; }
+    // the result is zeroed on the host before the tiles accumulate into it: it needs its real size
+    const size_t out_bytes = enc ? (size_t)16 * ((T - 1) / 4 + 1) * (H / 8) * (W / 8) * 2 : (size_t)3 * frames * 64 * H * W * 2;
+    return trace(eng, need, plan_only(13), out_bytes, [&](void* ws, size_t bytes, void* out) {
+      return enc ? svr2_vae_encode_tiled(&eng, in, 1, T, H, W, th, tw, oh, ow, slice, out, ws, bytes, nullptr)
+                 : svr2_vae_decode_tiled(&eng, in, 1, T, H, W, th, tw, oh, ow, slice, frames, out, ws, bytes, nullptr);
+    });
+  }
+  return 2;
 }

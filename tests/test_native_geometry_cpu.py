@@ -3,18 +3,15 @@ svr2_dit_forward builds per clip shape and svr2_dit_geometry returns) against th
 (oracle/dit_oracle.py: window boxes, window_token_index, rope_cos_sin_3b / _7b).  engine.cu is compiled with
 SVR2_HOST_TEST (tables kept in host memory) by nvcc's host compiler; skipped where nvcc is missing."""
 import math
-import os
-import shutil
 import subprocess
 
 import pytest
 import torch
 
+import native_trace
 from oracle import dit_oracle
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-pytestmark = pytest.mark.skipif(not os.path.exists(NVCC), reason="nvcc not available")
+pytestmark = native_trace.needs_nvcc
 
 # (regular, shifted) window counts of the SURVEY geometries (latent T, H/2, W/2)
 SURVEY_WINDOWS = {(1, 32, 32): (4, 9), (5, 68, 120): (75, 90), (3, 135, 240): (243, 300), (17, 135, 240): (324, 400),
@@ -23,12 +20,7 @@ SURVEY_WINDOWS = {(1, 32, 32): (4, 9), (5, 68, 120): (75, 90), (3, 135, 240): (2
 
 @pytest.fixture(scope="module")
 def dumper(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("geo") / "geometry_dump")
-    csrc = os.path.join(ROOT, "comfyui-seedvr2_videoupscaler_b200", "csrc")
-    r = subprocess.run([NVCC, "-std=c++17", "-O1", "-I", csrc, "-o", exe, os.path.join(ROOT, "tests", "native", "geometry_dump.cu"),
-                        "-Xlinker", "--unresolved-symbols=ignore-all"], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    return exe
+    return native_trace.harness(tmp_path_factory, "geometry_dump", link_svr2=False)
 
 
 def rope_freqs(variant, dtype):

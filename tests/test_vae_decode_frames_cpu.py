@@ -1,84 +1,27 @@
 """CPU: the VAE decode that returns only the first F output frames (svr2_vae_decode_frames / B200VideoVAE.decode(frames=F)).
-The native runtime (csrc/vae_engine.cu, compiled with SVR2_HOST_TEST through tests/native/vae_trace_frames.cu) must
+The native runtime (csrc/vae_engine.cu, compiled with SVR2_HOST_TEST through tests/native/vae_trace.cu) must
 enqueue the same kernels with the same scalar arguments as the Python module's sequencing (vae.py); F = 4T-3 must be
 exactly svr2_vae_decode; every layer after the last temporal upsampler must run on the slice's wanted frames only; the
 workspace plan must cover the run and be exact; F outside 1 .. 4T-3 must be refused."""
-import ctypes
-import importlib
-import os
-import shutil
-import subprocess
-
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-pytestmark = pytest.mark.skipif(not os.path.exists(NVCC), reason="nvcc not available")
-CSRC = os.path.join(ROOT, "comfyui-seedvr2_videoupscaler_b200", "csrc")
+import native_trace
+from native_trace import assert_same_ops, launches, run, summary
 
-
-def _compile(out_dir, name):
-    exe = str(out_dir / name)
-    r = subprocess.run([NVCC, "-std=c++17", "-O1", "-I", CSRC, "-o", exe, os.path.join(ROOT, "tests", "native", name + ".cu"),
-                        "-L", CSRC, "-lsvr2", "-Xlinker", "-rpath", "-Xlinker", CSRC], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
+pytestmark = native_trace.needs_nvcc
 
 
 @pytest.fixture(scope="module")
-def tracers(tmp_path_factory, pkg):
-    lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
-    lib.load()                                                     # builds nothing; fails loudly if libsvr2.so is missing
-    d = tmp_path_factory.mktemp("vae_frames")
-    return _compile(d, "vae_trace_frames"), _compile(d, "vae_trace")
+def tracer(tmp_path_factory):
+    return native_trace.harness(tmp_path_factory, "vae_trace")
 
 
 @pytest.fixture(scope="module")
-def cpu_vae(pkg, tmp_path_factory):
-    """The Python VAE module on the CPU with the kernel layer replaced by a recorder, and its weights manifest."""
-    lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
-    vae = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.vae")
-    mp = pytest.MonkeyPatch()
-    mp.setattr(lib, "device_check", lambda: (132, 9, 0))
-    eng = vae.B200VideoVAE(pkg.weights.synth_vae_state_dict(seed=1, dtype=torch.float16), device="cpu")
-    eng.native = False
-    log = []
-
-    def fmt(a):
-        if a is None:
-            return "p0"
-        if isinstance(a, ctypes.c_void_p):
-            return "p1" if a.value else "p0"
-        if isinstance(a, bool):
-            return str(int(a))
-        if isinstance(a, int):
-            return str(a)
-        if isinstance(a, float):
-            return "%.5g" % a
-        return "p1"                                                # ctypes.byref(...)
-
-    mp.setattr(lib, "call", lambda name, *args, flops=0.0, nbytes=0.0, tag="": log.append(" ".join([name] + [fmt(a) for a in args])))
-    mp.setattr(lib, "stream", lambda: None)
-    mp.setattr(lib, "_bf16c", lambda t, name: t)
-    mp.setattr(type(eng), "_require_cuda", lambda self, what: None)
-    mp.setattr(type(eng), "_frames_that_fit", lambda self, H, W, state_bytes_per_pixel=0: 10 ** 6)
-    mp.setattr(torch.cuda, "is_current_stream_capturing", lambda: False)
-    mp.setattr(torch.cuda, "memory_reserved", lambda d=None: 0)
-    mp.setattr(torch.cuda, "memory_allocated", lambda d=None: 0)
-    mp.setattr(torch.cuda, "empty_cache", lambda: None)
-    mp.setattr(torch.cuda, "get_device_properties", lambda d=None: type("P", (), {"total_memory": 1 << 40})())
-    manifest = str(tmp_path_factory.mktemp("vae_manifest") / "weights.txt")
-    with open(manifest, "w") as f:
-        for k, t in eng._native_tensors().items():
-            f.write(" ".join([k, str(max(t.ndim, 1))] + [str(n) for n in (t.shape if t.ndim else (1,))]) + "\n")
-    yield eng, log, manifest
-    mp.undo()
-
-
-def _native(exe, manifest, *args):
-    r = subprocess.run([exe, manifest, *map(str, args)], capture_output=True, text=True)
-    return r.returncode, r.stdout.strip().split("\n"), r.stderr
+def cpu_vae(tmp_path_factory):
+    """The recording Python VAE module and its weights manifest."""
+    with native_trace.recording_vae() as (eng, log):
+        yield eng, log, native_trace.write_manifest(eng, str(tmp_path_factory.mktemp("vae_manifest") / "weights.txt"))
 
 
 def _slices(T, slice_frames):
@@ -112,9 +55,8 @@ CASES = ([(T, 4, 6, 0, 4 * T - 3 - d) for T in (2, 3, 5) for d in range(4)]
 
 
 @pytest.mark.parametrize("T,h,w,slice_frames,F", CASES)
-def test_trimmed_decode_sequence_matches_python(cpu_vae, tracers, T, h, w, slice_frames, F):
+def test_trimmed_decode_sequence_matches_python(cpu_vae, tracer, T, h, w, slice_frames, F):
     eng, log, manifest = cpu_vae
-    trace_frames, trace_full = tracers
     del log[:]
     eng.set_causal_slicing(split_size=None if slice_frames == 0 else 4 * slice_frames)
     try:
@@ -123,21 +65,16 @@ def test_trimmed_decode_sequence_matches_python(cpu_vae, tracers, T, h, w, slice
         eng.set_causal_slicing(split_size=None)
     assert out.shape == (1, 3, F, 8 * h, 8 * w)
     want = list(log)
-    rc, lines, err = _native(trace_frames, manifest, T, h, w, slice_frames, F)
+    rc, lines, err = run(tracer, manifest, "frames", T, h, w, slice_frames, F)
     assert rc == 0, (rc, err[-2000:])
-    summary = lines.pop().split()
-    got = [ln.split(" | ")[0] for ln in lines]                     # drop the channel-stride suffix of the strided converters
-    assert len(got) == len(want), (len(got), len(want))
-    for i, (g, w_) in enumerate(zip(got, want)):
-        assert g == w_, f"op {i}: native `{g}` vs python `{w_}`"
-    need, touched, launches = int(summary[2]), int(summary[4]), int(summary[6])
+    need, touched, n_launches = summary(lines.pop())
+    assert_same_ops(lines, want)                                   # without the channel-stride suffix of the strided converters
     assert 0 < touched < need and need % 256 == 0                  # the dry run covers the run (a 256 B smaller one is refused)
-    lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
-    assert launches == sum(lib.KERNELS_PER_CALL.get(w_.split()[0], 1) for w_ in want)
+    assert n_launches == launches(want)
 
     # per slice: identical to the untrimmed decode up to the last temporal upsampler's shuffle, then every layer on `keep`
     keeps = _keeps(T, slice_frames, F)
-    rc, full, err = _native(trace_full, manifest, "dec", T, h, w, slice_frames)
+    rc, full, err = run(tracer, manifest, "dec", T, h, w, slice_frames)
     assert rc == 0, err[-2000:]
     full.pop()
     split = lambda ls: [[ln for ln in s.split("\n") if ln] for s in "\n".join(ls).split("svr2_ncdhw_to_ndhwc_bf16")[1:]]
@@ -165,34 +102,33 @@ def test_trimmed_decode_sequence_matches_python(cpu_vae, tracers, T, h, w, slice
 
 
 @pytest.mark.parametrize("T,h,w,slice_frames", [(2, 4, 6, 0), (3, 6, 10, 0), (5, 6, 10, 2), (6, 5, 7, 1), (1, 40, 24, 0)])
-def test_all_frames_is_the_untrimmed_decode(cpu_vae, tracers, T, h, w, slice_frames):
+def test_all_frames_is_the_untrimmed_decode(cpu_vae, tracer, T, h, w, slice_frames):
     """svr2_vae_decode_frames(F = 4T-3) enqueues exactly what svr2_vae_decode does, channel strides included, in a workspace
     of the same exact size."""
     _, _, manifest = cpu_vae
-    trace_frames, trace_full = tracers
-    rc, got, err = _native(trace_frames, manifest, T, h, w, slice_frames, 4 * T - 3)
+    rc, got, err = run(tracer, manifest, "frames", T, h, w, slice_frames, 4 * T - 3)
     assert rc == 0, err[-2000:]
-    rc, want, err = _native(trace_full, manifest, "dec", T, h, w, slice_frames)
+    rc, want, err = run(tracer, manifest, "dec", T, h, w, slice_frames)
     assert rc == 0, err[-2000:]
     assert got == want
 
 
 @pytest.mark.parametrize("T,F", [(2, 0), (2, 6), (2, -1), (1, 2), (5, 18)])
-def test_frames_out_of_range_are_refused(cpu_vae, tracers, T, F):
+def test_frames_out_of_range_are_refused(cpu_vae, tracer, T, F):
     eng, _, manifest = cpu_vae
-    rc, _, err = _native(tracers[0], manifest, T, 4, 6, 0, F)
+    rc, _, err = run(tracer, manifest, "frames", T, 4, 6, 0, F)
     assert rc == 3 and err.count(f"frames = {F}") == 2, (rc, err)   # the workspace query and the decode both refuse
     with pytest.raises(ValueError, match="frames"):
         eng.decode(torch.zeros(1, 16, T, 4, 6, dtype=torch.bfloat16), frames=F)
 
 
-def test_trimmed_workspace_of_the_flagship_shapes(cpu_vae, tracers):
+def test_trimmed_workspace_of_the_flagship_shapes(cpu_vae, tracer):
     """Exact decode workspaces of the 4K shard (latent 2 x 270 x 480: 5 frames decoded, 4 wanted) and of the 1080p clip
     (latent 5 x 135 x 240: 17 decoded, 16 wanted), untrimmed and trimmed."""
     _, _, manifest = cpu_vae
 
     def need(T, h, w, F):
-        rc, lines, err = _native(tracers[0], manifest, T, h, w, 0, F, "plan")
+        rc, lines, err = run(tracer, manifest, "frames", T, h, w, 0, F, "plan")
         assert rc == 0, err[-2000:]
         return int(lines[-1].split()[2])
 

@@ -5,51 +5,26 @@ sequence runs get them; the native runtime (csrc/vae_engine.cu, compiled with SV
 tests/native/vae_trace.cu) sets the fold on those convs in the first temporal slice of a clip and nowhere else, and its
 workspace plan does not change.  test_native_vae_cpu.py compares its launch sequence with the Python module's op by op."""
 import importlib
-import os
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-CSRC = os.path.join(ROOT, "comfyui-seedvr2_videoupscaler_b200", "csrc")
-pytestmark = pytest.mark.skipif(not os.path.exists(NVCC), reason="nvcc not available")
+import native_trace
+from native_trace import run, write_manifest
+
+pytestmark = native_trace.needs_nvcc
 EPI_FOLD_HEAD = 2048
 
 
 @pytest.fixture(scope="module")
-def cpu_vae(pkg):
-    lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
-    vae = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.vae")
-    mp = pytest.MonkeyPatch()
-    mp.setattr(lib, "device_check", lambda: (132, 9, 0))
-    eng = vae.B200VideoVAE(pkg.weights.synth_vae_state_dict(seed=1, dtype=torch.float16), device="cpu")
-    yield eng
-    mp.undo()
+def cpu_vae():
+    with native_trace.recording_vae() as (eng, _):
+        yield eng
 
 
 @pytest.fixture(scope="module")
-def tracers(tmp_path_factory, pkg):
-    importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib").load()
-    d = tmp_path_factory.mktemp("vae_fold")
-    exes = []
-    for name in ("vae_trace", "vae_trace_frames"):
-        exe = str(d / name)
-        r = subprocess.run([NVCC, "-std=c++17", "-O1", "-I", CSRC, "-o", exe, os.path.join(ROOT, "tests", "native", name + ".cu"),
-                            "-L", CSRC, "-lsvr2", "-Xlinker", "-rpath", "-Xlinker", CSRC], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-        exes.append(exe)
-    return exes
-
-
-def _manifest(eng, path, heads=True):
-    with open(path, "w") as f:
-        for k, t in eng._native_tensors().items():
-            if heads or not k.endswith(":head"):
-                f.write(" ".join([k, str(max(t.ndim, 1))] + [str(n) for n in (t.shape if t.ndim else (1,))]) + "\n")
-    return path
+def tracer(tmp_path_factory):
+    return native_trace.harness(tmp_path_factory, "vae_trace")
 
 
 def test_folded_weights_layout(cpu_vae, pkg):
@@ -105,10 +80,10 @@ def test_folded_weights_stay_views_after_a_device_move(pkg):
     assert len(live) == len(list(eng.buffers())) - len(heads)
 
 
-def _trace(exe, manifest, *args):
-    r = subprocess.run([exe, manifest, *map(str, args)], capture_output=True, text=True)
-    assert r.returncode == 0, (r.returncode, r.stderr[-2000:])
-    return r.stdout.strip().split("\n")
+def _trace(*args):
+    rc, lines, err = run(*args)
+    assert rc == 0, (rc, err[-2000:])
+    return lines
 
 
 def _convs_per_slice(lines):
@@ -127,10 +102,9 @@ def _convs_per_slice(lines):
     ("dec", 3, 6, 10, 0), ("dec", 5, 6, 10, 2), ("dec", 6, 5, 7, 1), ("dec", 1, 40, 24, 0),
     ("enc", 9, 48, 80, 0), ("enc", 17, 48, 80, 8), ("enc", 13, 32, 48, 4), ("enc", 1, 128, 160, 0),
 ])
-def test_fold_runs_in_the_first_slice_only(cpu_vae, tracers, tmp_path, direction, T, H, W, slice_frames):
-    trace = tracers[0]
-    with_heads = _trace(trace, _manifest(cpu_vae, str(tmp_path / "w.txt")), direction, T, H, W, slice_frames)
-    without = _trace(trace, _manifest(cpu_vae, str(tmp_path / "w0.txt"), heads=False), direction, T, H, W, slice_frames)
+def test_fold_runs_in_the_first_slice_only(cpu_vae, tracer, tmp_path, direction, T, H, W, slice_frames):
+    with_heads = _trace(tracer, write_manifest(cpu_vae, str(tmp_path / "w.txt")), direction, T, H, W, slice_frames)
+    without = _trace(tracer, write_manifest(cpu_vae, str(tmp_path / "w0.txt"), heads=False), direction, T, H, W, slice_frames)
     slices = _convs_per_slice(with_heads[:-1])
     assert len(slices) == (1 if slice_frames == 0 else len(_convs_per_slice(without[:-1])))
     for s, convs in enumerate(slices):
@@ -146,14 +120,13 @@ def test_fold_runs_in_the_first_slice_only(cpu_vae, tracers, tmp_path, direction
     assert with_heads[-1].split()[2] == without[-1].split()[2] and with_heads[-1].split()[6] == without[-1].split()[6]
 
 
-def test_workspace_of_the_flagship_shapes_unchanged(cpu_vae, tracers, tmp_path):
+def test_workspace_of_the_flagship_shapes_unchanged(cpu_vae, tracer, tmp_path):
     """The exact decode workspace of the 4K shard (latent 2 x 270 x 480, 4 of 5 frames) and of the 1080p clip (latent
     5 x 135 x 240, 16 of 17 frames), and of two encodes, with and without the folded weights: the fold allocates nothing."""
-    trace, trace_frames = tracers
-    m1, m0 = _manifest(cpu_vae, str(tmp_path / "w.txt")), _manifest(cpu_vae, str(tmp_path / "w0.txt"), heads=False)
+    m1, m0 = write_manifest(cpu_vae, str(tmp_path / "w.txt")), write_manifest(cpu_vae, str(tmp_path / "w0.txt"), heads=False)
     for T, h, w, F in ((2, 270, 480, 4), (5, 135, 240, 16)):
-        got = [_trace(trace_frames, m, T, h, w, 0, F, "plan")[-1] for m in (m1, m0)]
+        got = [_trace(tracer, m, "frames", T, h, w, 0, F, "plan")[-1] for m in (m1, m0)]
         assert got[0] == got[1], (T, h, w, got)
     for T, H, W in ((5, 96, 160), (17, 64, 96)):
-        got = [_trace(trace, m, "enc", T, H, W, 0)[-1].split()[2] for m in (m1, m0)]
+        got = [_trace(tracer, m, "enc", T, H, W, 0)[-1].split()[2] for m in (m1, m0)]
         assert got[0] == got[1], (T, H, W, got)

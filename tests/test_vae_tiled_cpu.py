@@ -1,81 +1,29 @@
 """CPU: the spatially tiled VAE passes of the native runtime (svr2_vae_encode_tiled / svr2_vae_decode_tiled, csrc/vae_engine.cu
-compiled with SVR2_HOST_TEST through tests/native/vae_tiled_trace.cu) against the Python module's tile-by-tile sequence
+compiled with SVR2_HOST_TEST through tests/native/vae_trace.cu) against the Python module's tile-by-tile sequence
 (vae.py B200VideoVAE._tiled, `.native = False`): the same tiles in the same order and every kernel with the same scalars,
 except two substitutions made exactly where expected — a tile's crop copy + input conversion is the windowed conversion
 (svr2_ncdhw_to_ndhwc_window reading the tile's rectangle of the clip), and a tile's final kernel +
 svr2_tile_accumulate_bf16 is the final kernel's seam variant (per temporal slice, at the tile's corner of the result).
 The exact workspace covers the run and a 256-byte smaller one is refused.  Also: the clip runner's tiling settings."""
-import ctypes
 import importlib
-import os
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-CSRC = os.path.join(ROOT, "comfyui-seedvr2_videoupscaler_b200", "csrc")
-needs_nvcc = pytest.mark.skipif(not os.path.exists(NVCC), reason="nvcc not available")
+import native_trace
+from native_trace import assert_same_ops, launches, needs_nvcc, run, summary
 
 
 @pytest.fixture(scope="module")
-def tracer(tmp_path_factory, pkg):
-    lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
-    lib.load()                                                     # builds nothing; fails loudly if libsvr2.so is missing
-    exe = str(tmp_path_factory.mktemp("vae_tiled") / "vae_tiled_trace")
-    r = subprocess.run([NVCC, "-std=c++17", "-O1", "-I", CSRC, "-o", exe, os.path.join(ROOT, "tests", "native", "vae_tiled_trace.cu"),
-                        "-L", CSRC, "-lsvr2", "-Xlinker", "-rpath", "-Xlinker", CSRC], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
+def tracer(tmp_path_factory):
+    return native_trace.harness(tmp_path_factory, "vae_trace")
 
 
 @pytest.fixture(scope="module")
-def cpu_vae(pkg, tmp_path_factory):
-    """The Python VAE module on the CPU with the kernel layer replaced by a recorder, and its weights manifest."""
-    lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
-    vae = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.vae")
-    mp = pytest.MonkeyPatch()
-    mp.setattr(lib, "device_check", lambda: (132, 9, 0))
-    eng = vae.B200VideoVAE(pkg.weights.synth_vae_state_dict(seed=1, dtype=torch.float16), device="cpu")
-    eng.native = False
-    log = []
-
-    def fmt(a):
-        if a is None:
-            return "p0"
-        if isinstance(a, ctypes.c_void_p):
-            return "p1" if a.value else "p0"
-        if isinstance(a, bool):
-            return str(int(a))
-        if isinstance(a, int):
-            return str(a)
-        if isinstance(a, float):
-            return "%.5g" % a
-        return "p1"
-
-    mp.setattr(lib, "call", lambda name, *args, flops=0.0, nbytes=0.0, tag="": log.append(" ".join([name] + [fmt(a) for a in args])))
-    mp.setattr(lib, "stream", lambda: None)
-    mp.setattr(lib, "_bf16c", lambda t, name: t)
-    mp.setattr(type(eng), "_require_cuda", lambda self, what: None)
-    mp.setattr(type(eng), "_frames_that_fit", lambda self, H, W, state_bytes_per_pixel=0: 10 ** 6)
-    mp.setattr(torch.cuda, "is_current_stream_capturing", lambda: False)
-    mp.setattr(torch.cuda, "memory_reserved", lambda d=None: 0)
-    mp.setattr(torch.cuda, "memory_allocated", lambda d=None: 0)
-    mp.setattr(torch.cuda, "empty_cache", lambda: None)
-    mp.setattr(torch.cuda, "get_device_properties", lambda d=None: type("P", (), {"total_memory": 1 << 40})())
-    manifest = str(tmp_path_factory.mktemp("vae_manifest") / "weights.txt")
-    with open(manifest, "w") as f:
-        for k, t in eng._native_tensors().items():
-            f.write(" ".join([k, str(max(t.ndim, 1))] + [str(n) for n in (t.shape if t.ndim else (1,))]) + "\n")
-    yield eng, log, manifest
-    mp.undo()
-
-
-def _native(exe, manifest, *args):
-    r = subprocess.run([exe, manifest, *map(str, args)], capture_output=True, text=True)
-    return r.returncode, r.stdout.strip().split("\n"), r.stderr
+def cpu_vae(tmp_path_factory):
+    """The recording Python VAE module and its weights manifest."""
+    with native_trace.recording_vae() as (eng, log):
+        yield eng, log, native_trace.write_manifest(eng, str(tmp_path_factory.mktemp("vae_manifest") / "weights.txt"))
 
 
 def _plan(encode, H, W, tile, ov):
@@ -116,7 +64,6 @@ def test_tiled_sequence_matches_python(cpu_vae, tracer, name):
     kind, T, H, W, tile, ov, split, frames = CASES[name]
     enc = kind == "enc"
     eng, log, manifest = cpu_vae
-    lib = importlib.import_module("comfyui_seedvr2_videoupscaler_b200.lib")
     del log[:]
     eng.set_causal_slicing(split_size=split)
     try:
@@ -131,17 +78,16 @@ def test_tiled_sequence_matches_python(cpu_vae, tracer, name):
     assert tuple(out.shape) == ((1, 16, F, H // 8, W // 8) if enc else (1, 3, F, 8 * H, 8 * W))
     want = list(log)
     slice_frames = 0 if split is None else (max(4, split // 4 * 4) if enc else max(1, split // 4))
-    rc, got, err = _native(tracer, manifest, kind, T, H, W, *tile, *ov, slice_frames, F)
+    rc, got, err = run(tracer, manifest, "tiled", kind, T, H, W, *tile, *ov, slice_frames, F)
     assert rc == 0, (rc, err[-2000:])
-    summary = got.pop().split()
-    need, touched, launches = int(summary[2]), int(summary[4]), int(summary[6])
+    need, touched, n_launches = summary(got.pop())
     assert 0 < touched < need and need % 256 == 0                  # the dry run covers the run (a 256 B smaller one is refused)
 
     whole, Hl, Wl, s, (lh, lw), tiles = _plan(enc, H, W, tile, ov)
     if whole:                                                       # the un-tiled pass, exactly
-        assert [ln.split(" | ")[0] for ln in got] == want
+        assert_same_ops(got, want)
         assert not any("accumulate" in ln for ln in want)
-        assert launches == sum(lib.KERNELS_PER_CALL.get(w_.split()[0], 1) for w_ in want)
+        assert n_launches == launches(want)
         return
     assert got[0] == f"svr2_tile_ramp_bf16 {'p1' if lh else 'p0'} {lh} {'p1' if lw else 'p0'} {lw} p0", got[0]
     Hr, Wr, C = Hl * s, Wl * s, (16 if enc else 3)
@@ -194,7 +140,7 @@ def test_tiled_sequence_matches_python(cpu_vae, tracer, name):
     assert gi == len(got) and tile_i == len(tiles)
     assert n_window == n_seam                                       # one of each per temporal slice
     n_acc = sum(w_.startswith("svr2_tile_accumulate_bf16") for w_ in want)
-    assert launches == sum(lib.KERNELS_PER_CALL.get(w_.split()[0], 1) for w_ in want) - n_acc + 1
+    assert n_launches == launches(want) - n_acc + 1
 
 
 @needs_nvcc
@@ -202,7 +148,7 @@ def test_tiled_arguments_refused(cpu_vae, tracer):
     _, _, manifest = cpu_vae
     for args in (("dec", 2, 8, 8, 0, 64, 8, 8, 0, 5), ("dec", 2, 8, 8, 64, 64, -8, 8, 0, 5), ("dec", 2, 8, 8, 32, 32, 8, 8, 0, 6),
                  ("enc", 5, 36, 40, 32, 32, 8, 8, 0, 0)):
-        rc, _, err = _native(tracer, manifest, *args)
+        rc, _, err = run(tracer, manifest, "tiled", *args)
         assert rc == 3 and "refused" in err, (args, rc, err)
 
 
@@ -213,7 +159,7 @@ def test_tiled_4k_needs_fit_one_gpu(cpu_vae, tracer):
     _, _, manifest = cpu_vae
 
     def need(*args):
-        rc, lines, err = _native(tracer, manifest, *args, "plan")
+        rc, lines, err = run(tracer, manifest, "tiled", *args, "plan")
         assert rc == 0, err[-2000:]
         return int(lines[-1].split()[2])
 
