@@ -232,13 +232,16 @@ __global__ void unpatchify_kernel(const __nv_bfloat16* __restrict__ in, int ld_i
 // ------------------------------------------------------------------ GroupNorm(32) per frame
 // Deterministic three-step reduction (no floating-point atomics, so results are bit-reproducible):
 //   1. stats   : block = slab of pixels of one frame, thread = 8 fixed channels; per-block partial
-//                (sum, sumsq) per group reduced in a fixed order -> partial[f][blk][32][2] (double)
+//                (sum, sumsq) per group reduced in a fixed order -> partial[f][blk][32][2] (double).
+//                The per-thread chains are fp64 too: var = E[x^2] - mean^2 cancels by (mean/std)^2, which an fp32
+//                chain of thousands of adds does not survive on offset or near-flat frames (a black frame after
+//                conv_in); bf16 squares are exact in fp32 (v * v below), so the sums are the only rounding.
 //   2. finalize: one block per frame sums the partials in block order and emits per-channel
 //                fp32 coefficients a = rstd*gamma, b = beta - mean*a
 //   3. apply   : y = silu(bf16(a*x + b)) (+ halo duplication of frame 0)
 __global__ void __launch_bounds__(256) groupnorm_stats_kernel(const __nv_bfloat16* __restrict__ x, int hw, int C,
                                                               int pix_per_block, double* __restrict__ partial) {
-  __shared__ float sm[256][4];
+  __shared__ double sm[256][4];
   const int f = blockIdx.y;
   const int cvec = C / 8;               // vectors per pixel
   const int cpg = C / 32;               // channels per group (4, 8, 16)
@@ -246,7 +249,7 @@ __global__ void __launch_bounds__(256) groupnorm_stats_kernel(const __nv_bfloat1
   const long long p1 = min((long long)hw, p0 + pix_per_block);
   const __nv_bfloat16* xf = x + (long long)f * hw * C;
   const int cv = threadIdx.x % cvec, pl = threadIdx.x / cvec, pstride = 256 / cvec;
-  float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;   // (s0,q0): channels 0-3 of the vector, (s1,q1): 4-7
+  double s0 = 0.0, q0 = 0.0, s1 = 0.0, q1 = 0.0;  // (s0,q0): channels 0-3 of the vector, (s1,q1): 4-7
   long long p = p0 + pl;
   for (; p + 3LL * pstride < p1; p += 4LL * pstride) {
     uint4 r[4];
@@ -278,8 +281,8 @@ __global__ void __launch_bounds__(256) groupnorm_stats_kernel(const __nv_bfloat1
       const int nv = cpg / 8;
       for (int l = 0; l < pstride; ++l)
         for (int v = g * nv; v < (g + 1) * nv; ++v) {
-          ds += (double)sm[l * cvec + v][0] + (double)sm[l * cvec + v][2];
-          dq += (double)sm[l * cvec + v][1] + (double)sm[l * cvec + v][3];
+          ds += sm[l * cvec + v][0] + sm[l * cvec + v][2];
+          dq += sm[l * cvec + v][1] + sm[l * cvec + v][3];
         }
     }
     double* dst = partial + (((long long)f * gridDim.x + blockIdx.x) * 32 + g) * 2;
@@ -324,11 +327,31 @@ __global__ void __launch_bounds__(256) groupnorm_finalize_kernel(const double* _
   }
 }
 
+// fixed-order tree over a block of 256 threads; every thread gets the totals
+__device__ __forceinline__ void block_sum2_256(double& ds, double& dq, double* sh_s, double* sh_q) {
+  sh_s[threadIdx.x] = ds;
+  sh_q[threadIdx.x] = dq;
+  __syncthreads();
+  for (int st = 128; st > 0; st >>= 1) {
+    if (threadIdx.x < st) {
+      sh_s[threadIdx.x] += sh_s[threadIdx.x + st];
+      sh_q[threadIdx.x] += sh_q[threadIdx.x + st];
+    }
+    __syncthreads();
+  }
+  ds = sh_s[0];
+  dq = sh_q[0];
+  __syncthreads();
+}
+
 // finalize from conv-epilogue partials: part [frames][slots][C/8] (sum0, sq0, sum1, sq1) per channel octet
 // (x/y: channels 0-3 of the octet, z/w: channels 4-7).  One block per (group, frame); every thread sums a
 // fixed strided subset of the slots in double, then a fixed-order shared-memory tree -> deterministic.
+// The partials are fp32 sums, so var = E[x^2] - mean^2 from them is off by ~1e-4 (mean/std)^2 of var.  A group with
+// mean^2 > 16 var (a near-flat or strongly offset group) is summed again from x, shifted by that mean:
+// sum (x - m~) and sum (x - m~)^2 do not cancel.  Only such groups pay the extra read of their channels.
 __global__ void __launch_bounds__(256) groupnorm_finalize_fused_kernel(const float4* __restrict__ part, int slots,
-                                                                       int hw, int C,
+                                                                       const __nv_bfloat16* __restrict__ x, int hw, int C,
                                                                        const __nv_bfloat16* __restrict__ gamma,
                                                                        const __nv_bfloat16* __restrict__ beta,
                                                                        float eps, float2* __restrict__ coef) {
@@ -353,18 +376,27 @@ __global__ void __launch_bounds__(256) groupnorm_finalize_fused_kernel(const flo
       }
     }
   }
-  sh_s[threadIdx.x] = ds;
-  sh_q[threadIdx.x] = dq;
-  __syncthreads();
-  for (int st = 128; st > 0; st >>= 1) {
-    if (threadIdx.x < st) {
-      sh_s[threadIdx.x] += sh_s[threadIdx.x + st];
-      sh_q[threadIdx.x] += sh_q[threadIdx.x + st];
-    }
-    __syncthreads();
-  }
+  block_sum2_256(ds, dq, sh_s, sh_q);
   const double n = (double)hw * cpg;
-  const double mean = sh_s[0] / n, var = sh_q[0] / n - mean * mean;
+  double mean = ds / n, var = dq / n - mean * mean;
+  if (16.0 * var < mean * mean) {                 // block-uniform
+    const float shift = (float)mean;
+    const int lg = cpg == 4 ? 0 : cpg == 8 ? 1 : 2;  // 4-channel chunks per pixel: 1 << lg
+    const __nv_bfloat16* xg = x + (long long)f * hw * C + g * cpg;
+    ds = 0.0;
+    dq = 0.0;
+    for (long long i = threadIdx.x; i < ((long long)hw << lg); i += 256) {
+      const uint2 r = *reinterpret_cast<const uint2*>(xg + (i >> lg) * C + (i & ((1 << lg) - 1)) * 4);
+      const float d0 = __uint_as_float(r.x << 16) - shift, d1 = __uint_as_float(r.x & 0xffff0000u) - shift;
+      const float d2 = __uint_as_float(r.y << 16) - shift, d3 = __uint_as_float(r.y & 0xffff0000u) - shift;
+      ds += (d0 + d1) + (d2 + d3);
+      dq += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
+    }
+    block_sum2_256(ds, dq, sh_s, sh_q);
+    const double dm = ds / n;
+    mean = (double)shift + dm;
+    var = dq / n - dm * dm;
+  }
   const float rstd = rsqrtf(fmaxf((float)var, 0.f) + eps);
   if (threadIdx.x < cpg) {
     const int c = g * cpg + threadIdx.x;
@@ -824,6 +856,8 @@ extern "C" int svr2_groupnorm_bf16(const void* x, void* y, int frames, int hw, i
                                    double* scratch, int64_t scratch_bytes, void* stream) {
   if (C % 32 || (C / 32 != 4 && C / 32 != 8 && C / 32 != 16))
     return set_error(SVR2_ERR_ARG, "groupnorm: C must be 128, 256 or 512");
+  if (out_dup_head && out_t_pad != 2)        // the apply kernel copies frame 0 into exactly two halo frames
+    return set_error(SVR2_ERR_ARG, "groupnorm: out_dup_head needs out_t_pad == 2");
   cudaStream_t s = (cudaStream_t)stream;
   int blocks_x = (int)((hw + 4095) / 4096);
   if (blocks_x < 1) blocks_x = 1;
@@ -856,9 +890,12 @@ extern "C" int svr2_groupnorm_from_stats_bf16(const void* x, void* y, int frames
                                               void* stream) {
   if (C % 32 || (C / 32 != 4 && C / 32 != 8 && C / 32 != 16))
     return set_error(SVR2_ERR_ARG, "groupnorm: C must be 128, 256 or 512");
+  if (out_dup_head && out_t_pad != 2)        // the apply kernel copies frame 0 into exactly two halo frames
+    return set_error(SVR2_ERR_ARG, "groupnorm: out_dup_head needs out_t_pad == 2");
   cudaStream_t s = (cudaStream_t)stream;
   float2* coef = (float2*)coef_scratch;
-  groupnorm_finalize_fused_kernel<<<dim3(32, frames), 256, 0, s>>>((const float4*)stat_partial, stat_slots, hw, C,
+  groupnorm_finalize_fused_kernel<<<dim3(32, frames), 256, 0, s>>>((const float4*)stat_partial, stat_slots,
+                                                                   (const __nv_bfloat16*)x, hw, C,
                                                          (const __nv_bfloat16*)gamma, (const __nv_bfloat16*)beta, eps,
                                                          coef);
   int rc = check_launch("groupnorm_finalize_fused");

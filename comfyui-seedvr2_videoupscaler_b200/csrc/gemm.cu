@@ -1596,6 +1596,8 @@ static int conv3d_impl(const void* x, int T_in_total, int H, int W, int Cin, con
   if (Cin % 64) return set_error(SVR2_ERR_ARG, "svr2_conv3d_bf16: Cin must be a multiple of 64 (pad channels)");
   if (Cout % 8 || ldc % 8) return set_error(SVR2_ERR_ARG, "svr2_conv3d_bf16: Cout/ldc must be multiples of 8");
   if (stride_hw != 1 && stride_hw != 2) return set_error(SVR2_ERR_ARG, "stride_hw must be 1 or 2");
+  if (out_dup_head && out_t_pad != 2)        // the epilogue copies frame 0 into exactly two halo frames
+    return set_error(SVR2_ERR_ARG, "svr2_conv3d_bf16: out_dup_head needs out_t_pad == 2");
   const int H_out = stride_hw == 1 ? H : H / 2, W_out = stride_hw == 1 ? W : W / 2;
   if (stride_hw == 2 && ((H | W) & 1)) return set_error(SVR2_ERR_ARG, "stride-2 conv needs even H, W");
   bool swap;
@@ -1704,6 +1706,8 @@ extern "C" int svr2_upsample_shuffle_bf16(const void* x, int F, int H, int W, in
   const int N = 4 * z * C, M = F * H * W;
   const int bn = C >= 256 ? 256 : 128;
   if (C % bn) return set_error(SVR2_ERR_ARG, "svr2_upsample_shuffle_bf16: C must be a multiple of 128");
+  if (out_dup_head && out_t_pad != 2)
+    return set_error(SVR2_ERR_ARG, "svr2_upsample_shuffle_bf16: out_dup_head needs out_t_pad == 2");
   CUtensorMap ta, tb;
   uint64_t da[2] = {(uint64_t)C, (uint64_t)M}, sa[1] = {(uint64_t)C * 2};
   uint32_t ba[2] = {BLOCK_K, BLOCK_M};
