@@ -333,6 +333,55 @@ __global__ void __launch_bounds__(256) blend_overlap_f32_kernel(const float4* __
   }
 }
 
+// The rank-seam cross-fade of a streamed multi-GPU run: fp32 open tail `prev` against a bf16 chunk head `cur`, the
+// fp32 value of blend_overlap_f32_kernel on (prev, cur.float()) written to out_f (when not NULL) and its CLI byte
+// (to_byte: * 255 without FMA, truncated, saturating, NaN -> 0) to out_b (when not NULL), in one pass.  Frames have
+// any element count: with `vec`, the elements from the first multiple of 4 of the flat index on are moved 4 at a time
+// (16-byte fp32, 8-byte bf16 and 4-byte u8 accesses, all aligned together), the few before and after one at a time.
+template <bool F, bool B>
+__device__ __forceinline__ void blend_u8_one(const float* prev, const __nv_bfloat16* cur, float* out_f, uint8_t* out_b,
+                                             long long e, float wp, float wc) {
+  const float v = __fadd_rn(__fmul_rn(prev[e], wp), __fmul_rn(bf2f(cur[e]), wc));
+  if (F) out_f[e] = v;
+  if (B) out_b[e] = (uint8_t)to_byte(v);
+}
+
+template <bool F, bool B>
+__global__ void __launch_bounds__(256) blend_overlap_u8_kernel(const float* __restrict__ prev,
+                                                               const __nv_bfloat16* __restrict__ cur,
+                                                               float* __restrict__ out_f, uint8_t* __restrict__ out_b,
+                                                               const float* __restrict__ w_prev,
+                                                               const float* __restrict__ w_cur, long long frame_elems,
+                                                               int vec) {
+  const int f = blockIdx.y;
+  const float wp = w_prev[f], wc = w_cur[f];
+  const long long base = (long long)f * frame_elems;
+  const long long lead = vec ? min((4 - base % 4) % 4, frame_elems) : frame_elems;   // elements before the body
+  const long long nvec = (frame_elems - lead) / 4;
+  const long long stride = (long long)gridDim.x * 256, t0 = (long long)blockIdx.x * 256 + threadIdx.x;
+  for (long long i = t0; i < nvec; i += stride) {
+    const long long e = base + lead + 4 * i;
+    const float4 a = *reinterpret_cast<const float4*>(prev + e);
+    const uint2 b = *reinterpret_cast<const uint2*>(cur + e);
+    const float av[4] = {a.x, a.y, a.z, a.w};
+    const float bv[4] = {__uint_as_float(b.x << 16), __uint_as_float(b.x & 0xffff0000u), __uint_as_float(b.y << 16),
+                         __uint_as_float(b.y & 0xffff0000u)};
+    float v[4];
+    uint32_t word = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      v[k] = __fadd_rn(__fmul_rn(av[k], wp), __fmul_rn(bv[k], wc));
+      word |= to_byte(v[k]) << (8 * k);
+    }
+    if (F) *reinterpret_cast<float4*>(out_f + e) = make_float4(v[0], v[1], v[2], v[3]);
+    if (B) *reinterpret_cast<uint32_t*>(out_b + e) = word;
+  }
+  // the scalar elements: [0, lead) and [lead + 4 nvec, frame_elems) of the frame
+  const long long rest = frame_elems - 4 * nvec;
+  for (long long i = t0; i < rest; i += stride)
+    blend_u8_one<F, B>(prev, cur, out_f, out_b, base + (i < lead ? i : 4 * nvec + i), wp, wc);
+}
+
 // Spatially tiled VAE (tiled_encode / tiled_decode, attn_video_vae.py:1302-1630): one tile accumulated into the running
 // result with separable edge weights, in bf16 with torch's in-place op order — tile.mul_(wh).mul_(ww); result += tile;
 // count.addcmul_(wh, ww) — i.e. every product / sum is rounded to bf16 where the reference rounds it.
@@ -580,6 +629,30 @@ extern "C" int svr2_blend_overlap_f32(const float* prev_tail, const float* cur_h
   blend_overlap_f32_kernel<<<dim3(bx, overlap), 256, 0, (cudaStream_t)stream>>>((const float4*)prev_tail, (const float4*)cur_head,
                                                                                  (float4*)out, w_prev, w_cur, vec);
   return check_launch("blend_overlap_f32");
+}
+
+extern "C" int svr2_blend_overlap_u8(const float* prev_tail, const void* cur_head, float* out_f32, void* out_u8,
+                                     const float* w_prev, const float* w_cur, int overlap, int64_t frame_elems,
+                                     void* stream) {
+  if (overlap <= 0 || frame_elems <= 0) return set_error(SVR2_ERR_ARG, "svr2_blend_overlap_u8: empty input");
+  if (overlap > 65535) return set_error(SVR2_ERR_ARG, "svr2_blend_overlap_u8: overlap <= 65535");
+  if (!prev_tail || !cur_head || !w_prev || !w_cur || (!out_f32 && !out_u8))
+    return set_error(SVR2_ERR_ARG, "svr2_blend_overlap_u8: null input, or neither output given");
+  const int vec = ((uintptr_t)prev_tail % 16) == 0 && ((uintptr_t)cur_head % 8) == 0 && ((uintptr_t)out_f32 % 16) == 0 &&
+                  ((uintptr_t)out_u8 % 4) == 0;
+  int bx = grid_for(vec ? frame_elems / 4 + 1 : frame_elems, 256, 8) / overlap;
+  if (bx < 1) bx = 1;
+  const dim3 grid(bx, overlap);
+  cudaStream_t s = (cudaStream_t)stream;
+  const __nv_bfloat16* cur = (const __nv_bfloat16*)cur_head;
+  uint8_t* ob = (uint8_t*)out_u8;
+  if (out_f32 && out_u8)
+    blend_overlap_u8_kernel<true, true><<<grid, 256, 0, s>>>(prev_tail, cur, out_f32, ob, w_prev, w_cur, frame_elems, vec);
+  else if (out_f32)
+    blend_overlap_u8_kernel<true, false><<<grid, 256, 0, s>>>(prev_tail, cur, out_f32, ob, w_prev, w_cur, frame_elems, vec);
+  else
+    blend_overlap_u8_kernel<false, true><<<grid, 256, 0, s>>>(prev_tail, cur, out_f32, ob, w_prev, w_cur, frame_elems, vec);
+  return check_launch("blend_overlap_u8");
 }
 
 extern "C" int svr2_tile_accumulate_bf16(const void* tile, int64_t tile_plane_stride, int tile_row_stride, int planes,

@@ -109,6 +109,7 @@ SIGNATURES = {
     "svr2_sample_to_image_u8": [_P, _P, _P, c_int, c_int64, _P],
     "svr2_blend_overlap_bf16": [_P, _P, _P, _P, _P, c_int, c_int64, _P],
     "svr2_blend_overlap_f32": [_P, _P, _P, _P, _P, c_int, c_int64, _P],
+    "svr2_blend_overlap_u8": [_P, _P, _P, _P, _P, _P, c_int, c_int64, _P],
     "svr2_tile_accumulate_bf16": [_P, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P],
     "svr2_tile_normalize_bf16": [_P, _P, c_int, c_int64, _P],
     "svr2_tile_ramp_bf16": [_P, c_int, _P, c_int, _P],

@@ -208,17 +208,34 @@ class SeedVR2Engine:
         with numpy's truncation, formatted in the same pass (``color_fix.sample_to_image_u8``)."""
         if out_dtype not in (torch.bfloat16, torch.uint8):
             raise ValueError(f"out_dtype must be torch.bfloat16 or torch.uint8, got {out_dtype}")
-        u8 = out_dtype == torch.uint8
+        return SeedVR2Engine.format_image(*SeedVR2Engine.correct_clip(sample, style, src, color_correction), out_dtype)
+
+    @staticmethod
+    def correct_clip(sample: torch.Tensor, style: torch.Tensor, src: Optional[torch.Tensor] = None,
+                     color_correction: str = "none"):
+        """``finish_clip`` up to the image format: (the colour-corrected sample, the bf16 RGBA image (T,H,W,4) whose
+        channel 3 holds the alpha upscaled from ``src``, or None without ``src``)."""
         if src is None:
             if color_correction != "none":
                 sample = color_fix.apply_color_correction(sample, style, color_correction)
-            return color_fix.sample_to_image_u8(sample) if u8 else color_fix.sample_to_image(sample)   # t h w c
+            return sample, None
         sample = sample.to(torch.bfloat16).contiguous()
         T, _, H, W = sample.shape
         image = torch.empty(T, H, W, 4, device=sample.device, dtype=torch.bfloat16)
         alpha.upscale_into_image(src, sample, image)
         if color_correction != "none":
             sample = color_fix.apply_color_correction(sample, style, color_correction)
+        return sample, image
+
+    @staticmethod
+    def format_image(sample: torch.Tensor, image: Optional[torch.Tensor] = None,
+                     out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+        """The [0,1] image format (T,H,W,3) of a corrected sample, or (T,H,W,4) written into the RGBA ``image`` of
+        ``correct_clip`` (bf16); ``torch.uint8``: the CLI's 8-bit frames of it.  Per frame, so any frame range of a
+        ``correct_clip`` result can be formatted on its own."""
+        u8 = out_dtype == torch.uint8
+        if image is None:
+            return color_fix.sample_to_image_u8(sample) if u8 else color_fix.sample_to_image(sample)   # t h w c
         return color_fix.sample_to_image_u8(sample, image) if u8 else color_fix.sample_to_image_rgba(sample, image)
 
     @torch.no_grad()
@@ -397,14 +414,17 @@ class SeedVR2Engine:
 
     def _final_slices(self, frames, batch_size, temporal_overlap, seed, color_correction, resolution, max_resolution,
                       keep_alpha, input_noise_scale, latent_noise_scale, uniform_batch_size, prepend_frames,
-                      out_dtype=torch.bfloat16, tiling=None):
-        """``final_slices`` over the engine's batches: per batch, the phase-4 images (on the device) it made final."""
+                      out_dtype=torch.bfloat16, tiling=None, finish=None):
+        """``final_slices`` over the engine's batches: per batch, the phase-4 images (on the device) it made final.
+        ``frames`` may be a ``FrameSource`` already (``prepend_frames`` then plays no part); ``finish(sample, style,
+        src)`` replaces ``finish_clip`` as phase 4 (src: the RGBA input frames of the slice with ``keep_alpha``, else
+        None)."""
         from . import shard
         input_noise_scale = gen_noise.check_scale("input_noise_scale", input_noise_scale)
         latent_noise_scale = gen_noise.check_scale("latent_noise_scale", latent_noise_scale)
         if prepend_frames < 0:
             raise ValueError(f"prepend_frames must be >= 0, got {prepend_frames}")
-        source = FrameSource(frames, prepend_frames)
+        source = frames if isinstance(frames, FrameSource) else FrameSource(frames, prepend_frames)
         rgba = keep_alpha and source.channels == 4
         gen = gen_noise.input_generator(seed, self.device) if input_noise_scale > 0 else None
         noise_kw = dict(input_noise_scale=input_noise_scale, latent_noise_scale=latent_noise_scale, input_generator=gen)
@@ -420,6 +440,8 @@ class SeedVR2Engine:
 
         def post(sample, style):
             style, src = style if rgba else (style, None)
+            if finish is not None:
+                return finish(sample, style, src)
             return self.finish_clip(sample, style, src, color_correction=color_correction, out_dtype=out_dtype)
 
         return final_slices(source, batch_size, temporal_overlap, clip, shard.blend_overlap, post)
@@ -496,6 +518,30 @@ class FrameSource:
             if pos >= b:
                 break
         return pieces[0] if len(pieces) == 1 else torch.cat(pieces, 0)
+
+
+class RangeSource(FrameSource):
+    """Frames [a, b) of a video with ``prepend`` = p mirrored frames put in front (``pad_video_temporal(video, p,
+    prepend=True)``, ``total`` + p frames in all), as a ``FrameSource`` numbered from 0: one rank's share of a
+    multi-GPU run.  ``read(start, end)`` returns the source frames [start, end) (a tensor or an iterable of chunks)
+    and is called once.  A range that reaches into the mirrored frames reads the source from its start, and at least
+    the p + 1 frames the mirror is made of, even when the range is shorter."""
+
+    def __init__(self, read, total: int, a: int, b: int, prepend: int = 0):
+        p = prepend
+        if a < p:
+            self._src, self._off = FrameSource(read(0, max(b - p, min(p + 1, total))), prepend=p), a
+        else:
+            self._src, self._off = FrameSource(read(a - p, b - p)), 0
+        self._len = b - a
+        self.channels = self._src.channels
+
+    def fill(self, n: int) -> int:
+        n = min(n, self._len)
+        return max(0, min(n, self._src.fill(n + self._off) - self._off))
+
+    def take(self, a: int, b: int) -> torch.Tensor:
+        return self._src.take(a + self._off, b + self._off)
 
 
 def _frames(x, sl: slice):

@@ -387,6 +387,14 @@ int svr2_blend_overlap_bf16(const void* prev_tail, const void* cur_head, void* o
 int svr2_blend_overlap_f32(const float* prev_tail, const float* cur_head, float* out, const float* w_prev,
                            const float* w_cur, int overlap, int64_t frame_elems, void* stream);
 
+/* The rank-seam cross-fade of a streamed multi-GPU run: fp32 open tail prev_tail [overlap, frame_elems] against a bf16
+ * chunk head cur_head of the same shape.  out_f32 (NULL: not written) receives exactly what svr2_blend_overlap_f32
+ * gives for (prev_tail, cur_head as fp32); out_u8 (NULL: not written) the reference CLI's byte of that value, the rule
+ * of svr2_sample_to_image_u8 (fp32 * 255 without FMA, truncated; outside [0, 255] saturates, NaN gives 0).  One pass
+ * writes both; frame_elems is any positive count (no padding needed).  At least one output must be given. */
+int svr2_blend_overlap_u8(const float* prev_tail, const void* cur_head, float* out_f32, void* out_u8, const float* w_prev,
+                          const float* w_cur, int overlap, int64_t frame_elems, void* stream);
+
 /* ---- Spatially tiled VAE seams (VideoAutoencoderKL.tiled_encode / tiled_decode, attn_video_vae.py:1302-1630; optional,
  * off in every BASELINE config).  Accumulate one tile [planes, eff_h, eff_w] (plane / row strides in elements) into
  * result [planes, H, W] at (y0, x0) with separable bf16 edge weights, and its weight into count [H, W]; rounding points
