@@ -149,15 +149,16 @@ __global__ void __launch_bounds__(256) adain_apply_kernel(const __nv_bfloat16* _
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// sRGB <-> CIELAB (D65), color_fix.py:299-321, 368-474
+// sRGB <-> CIELAB (D65), color_fix.py:299-321, 368-474.  epsilon^3 and kappa are the fp32 casts of the reference's
+// double constants ((6/29)^3 = 216/24389, (29/3)^3 = 24389/27); cubing the fp32 quotients instead gives values one
+// ulp higher (0.008856453, 903.2964), which shifts every dark pixel's L*, a*, b*.
+constexpr float kLabEps3 = (float)(216.0 / 24389.0);
+constexpr float kLabKappa = (float)(24389.0 / 27.0);
 __device__ __forceinline__ float lab_f(float t) {
-  const float e3 = (6.0f / 29.0f) * (6.0f / 29.0f) * (6.0f / 29.0f);
-  const float kappa = (29.0f / 3.0f) * (29.0f / 3.0f) * (29.0f / 3.0f);
-  return t > e3 ? powf(t, 1.0f / 3.0f) : (t * kappa + 16.0f) / 116.0f;
+  return t > kLabEps3 ? powf(t, 1.0f / 3.0f) : (t * kLabKappa + 16.0f) / 116.0f;
 }
 __device__ __forceinline__ float lab_finv(float f) {
-  const float kappa = (29.0f / 3.0f) * (29.0f / 3.0f) * (29.0f / 3.0f);
-  return f > (6.0f / 29.0f) ? powf(f, 3.0f) : (f * 116.0f - 16.0f) / kappa;
+  return f > (6.0f / 29.0f) ? powf(f, 3.0f) : (f * 116.0f - 16.0f) / kLabKappa;
 }
 
 // rgb: [T,3,hw] bf16 in [-1,1]  ->  lab: [3][T*hw] fp32 (channel-major: each channel is one sortable array)
@@ -500,6 +501,7 @@ extern "C" int svr2_wavelet_level_f32(const void* img, int img_bf16, float* low,
 extern "C" int svr2_adain_bf16(const void* content, const void* style, void* out, int planes, int64_t hw,
                                float* stats_scratch, void* stream) {
   if (planes <= 0 || hw <= 0) return set_error(SVR2_ERR_ARG, "svr2_adain_bf16: empty input");
+  if (planes > 65535) return set_error(SVR2_ERR_ARG, "svr2_adain_bf16: planes <= 65535");   // the apply grid's y
   if (!stats_scratch) return set_error(SVR2_ERR_ARG, "svr2_adain_bf16: stats scratch (planes * 4 floats) required");
   cudaStream_t s = (cudaStream_t)stream;
   adain_stats_kernel<<<2 * planes, 1024, 0, s>>>((const __nv_bfloat16*)content, (const __nv_bfloat16*)style, hw,

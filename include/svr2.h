@@ -336,7 +336,11 @@ int svr2_wavelet_level_bf16(const void* img, void* low, void* high, const void* 
 int svr2_wavelet_level_f32(const void* img, int img_bf16, float* low, float* high, const float* add_to, float* out,
                            int planes, int H, int W, int radius, int first, void* stream);
 /* adaptive_instance_normalization (color_fix.py:72-119): per plane, out = (c - mean_c) / std_c * std_s + mean_s with
- * unbiased variance, eps 1e-5 and the reference's bf16 rounding points.  stats_scratch: planes * 4 floats. */
+ * unbiased variance, eps 1e-5 and the reference's bf16 rounding points; planes <= 65535.  stats_scratch: planes * 4
+ * floats; the call
+ * leaves in it (mean, std) as float pairs, content planes first, then style planes.  A plane of one pixel (hw = 1),
+ * whose unbiased variance torch returns as NaN, has variance 0 here: std = bf16(sqrt(bf16(eps))), so every content
+ * pixel maps to its style plane's mean instead of NaN. */
 int svr2_adain_bf16(const void* content, const void* style, void* out, int planes, int64_t hw, float* stats_scratch,
                     void* stream);
 /* _rgb_to_lab_batch (color_fix.py:299-321, 368-413): rgb [frames,3,hw] bf16 in [-1,1] -> lab [3][frames*hw] fp32 */

@@ -49,31 +49,6 @@ def test_color_fix_vs_reference_golden(cf, name):
     assert frac_equal(l, ref) > 0.98 and psnr(l, ref) > 55.0, (frac_equal(l, ref), psnr(l, ref))
 
 
-def test_color_fix_medium_size_vs_oracle(cf):
-    """A 2 x 270 x 480 clip (latent size of the 4K shard): all five dilations un-capped."""
-    content, style = color_inputs(2, 270, 480, seed=11)
-    c, s = content.cuda(), style.cuda()
-    w = cf.wavelet_reconstruction(c, s)
-    assert frac_equal(w, color_oracle.wavelet_reconstruction(content, style)) > 0.999
-    a = cf.adaptive_instance_normalization(c, s)
-    assert psnr(a, color_oracle.adaptive_instance_normalization(content, style)) > 60.0
-    l = cf.lab_color_transfer(c, s, None)
-    lo = color_oracle.lab_color_transfer(content, style)
-    assert psnr(l, lo) > 55.0 and frac_equal(l, lo) > 0.98
-    # luminance_weight = 1 keeps the content L* (color_fix.py:340-342)
-    l1 = cf.lab_color_transfer(c, s, None, luminance_weight=1.0)
-    assert psnr(l1, color_oracle.lab_color_transfer(content, style, luminance_weight=1.0)) > 55.0
-
-
-def test_color_fix_odd_sizes_vs_oracle(cf):
-    """Odd width / height (the two-pixels-per-thread wavelet kernel's ragged last column, capped dilations)."""
-    content, style = color_inputs(2, 37, 53, seed=13)
-    c, s = content.cuda(), style.cuda()
-    assert frac_equal(cf.wavelet_reconstruction(c, s), color_oracle.wavelet_reconstruction(content, style)) > 0.999
-    assert psnr(cf.adaptive_instance_normalization(c, s), color_oracle.adaptive_instance_normalization(content, style)) > 60.0
-    assert psnr(cf.lab_color_transfer(c, s, None), color_oracle.lab_color_transfer(content, style)) > 55.0
-
-
 def test_histogram_match_is_exact_rank_mapping(svr2lib):
     """Size-independent properties at 4M elements: the output is a permutation of the reference values and
     preserves the order of the source."""
