@@ -138,9 +138,10 @@ __global__ void alpha_finalize_kernel(AlphaHdr* __restrict__ hdr, long long n_al
   hdr->radius = hdr->binary ? 2 : 3;
 }
 
-// F.interpolate(alpha, (H, W), bicubic, antialias=True).clamp(0, 1) in fp32 (:342-348), the taps of torch's CUDA
-// kernel (horizontal taps first, then rows) as in pre.cu's resize; one output channel, input read through the
-// channel stride of the frames.
+// F.interpolate(alpha, (H, W), bicubic, antialias=True).clamp(0, 1) in fp32 (:342-348) as torch's CUDA kernel
+// computes it on the reference's GPU tensor: its tap tables (aa_resize.cuh) and its accumulation (horizontal taps
+// first, then rows, each a product and an fma chain), as in pre.cu's resize; one output channel, input read through
+// the channel stride of the frames.
 template <typename T>
 __global__ void __launch_bounds__(256) alpha_resize_kernel(const T* __restrict__ in, int channels, int h, int w,
                                                            float* __restrict__ out, int H, int W, int K,
@@ -158,9 +159,9 @@ __global__ void __launch_bounds__(256) alpha_resize_kernel(const T* __restrict__
   float acc = 0.f;
   for (int j = 0; j < ny; ++j) {
     const T* row = base + ((long long)(y0 + j) * w + x0) * channels;
-    float r = load_bf16_rounded<T>(row) * wx[0];
-    for (int i = 1; i < nx; ++i) r += load_bf16_rounded<T>(row + (long long)i * channels) * wx[i];
-    acc = (j == 0) ? r * wy[j] : acc + r * wy[j];
+    float r = __fmul_rn(load_bf16_rounded<T>(row), wx[0]);
+    for (int i = 1; i < nx; ++i) r = __fmaf_rn(load_bf16_rounded<T>(row + (long long)i * channels), wx[i], r);
+    acc = (j == 0) ? __fmul_rn(r, wy[j]) : __fmaf_rn(r, wy[j], acc);
   }
   out[((long long)t * H + oy) * W + ox] = fminf(fmaxf(acc, 0.f), 1.f);
 }
@@ -433,7 +434,7 @@ extern "C" int svr2_alpha_upscale(const void* alpha_src, int src_dtype, int src_
   if (out_kind < 0 || out_kind > 2) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: out_kind 0 | 1 | 2");
   if (!alpha_src || !rgb_up || !out) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: null pointer");
   const Layout l = layout(frames, h, w, H, W);
-  if (l.K > kMaxTaps) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: down-scale factor too large (> 7x)");
+  if (l.K > kMaxTaps) return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: down-scale factor above 7.5 (more than 31 taps)");
   if (!scratch || scratch_bytes < (int64_t)l.total)
     return set_error(SVR2_ERR_ARG, "svr2_alpha_upscale: scratch too small (svr2_alpha_upscale_scratch_bytes)");
   cudaStream_t s = (cudaStream_t)stream;

@@ -5,7 +5,9 @@
 //                                      weights normalised, fp32 accumulation, horizontal taps first)
 //   -> bf16 -> clamp(0,1) -> pad to multiples of 16 with zeros (DivisiblePad, divisible_crop.py:43-80)
 //   -> Normalize(0.5, 0.5) -> t c h w -> c t h w
-// The tap tables are built on the device (aa_resize.cuh).
+// The reference runs this Compose on the GPU (generation_phases.py:236, 380-413), so the resize is torch's CUDA
+// kernel: the tap tables are built on the device with its fp32 arithmetic (aa_resize.cuh) and the accumulation
+// follows its order, so the result equals torch's bit for bit.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -40,7 +42,8 @@ __global__ void __launch_bounds__(256) resize_kernel(const T* __restrict__ in, _
     const float* wx = xw + (long long)ox * K;
     const float* wy = yw + (long long)oy * K;
     // one pass over the taps for all three channels: each weight is fetched once, the per-channel accumulation
-    // order (horizontal taps left to right, then rows top to bottom) is that of torch's kernel
+    // (horizontal taps left to right, then rows top to bottom, a product and then an fma chain for each) is that of
+    // torch's kernel (interpolate_aa_single_dim)
     const long long cstride = channels_last ? 1 : (long long)h * w;
     const long long pstride = channels_last ? cin : 1;
     const T* base = in + (channels_last ? ((long long)t * h * w) * cin : ((long long)t * 3) * h * w);
@@ -50,15 +53,15 @@ __global__ void __launch_bounds__(256) resize_kernel(const T* __restrict__ in, _
       const float w0 = wx[0];
       float r[3];
 #pragma unroll
-      for (int c = 0; c < 3; ++c) r[c] = load_bf16_rounded<T>(row + c * cstride) * w0;
+      for (int c = 0; c < 3; ++c) r[c] = __fmul_rn(load_bf16_rounded<T>(row + c * cstride), w0);
       for (int i = 1; i < nx; ++i) {
         const float wi = wx[i];
 #pragma unroll
-        for (int c = 0; c < 3; ++c) r[c] += load_bf16_rounded<T>(row + i * pstride + c * cstride) * wi;
+        for (int c = 0; c < 3; ++c) r[c] = __fmaf_rn(load_bf16_rounded<T>(row + i * pstride + c * cstride), wi, r[c]);
       }
       const float wj = wy[j];
 #pragma unroll
-      for (int c = 0; c < 3; ++c) acc[c] = (j == 0) ? r[c] * wj : acc[c] + r[c] * wj;
+      for (int c = 0; c < 3; ++c) acc[c] = (j == 0) ? __fmul_rn(r[c], wj) : __fmaf_rn(r[c], wj, acc[c]);
     }
 #pragma unroll
     for (int c = 0; c < 3; ++c) res[c] = rn(acc[c]);
@@ -93,7 +96,7 @@ extern "C" int svr2_resize_bicubic_aa_bf16(const void* in, int in_dtype, int cha
   if (frames > 65535) return set_error(SVR2_ERR_ARG, "svr2_resize: at most 65535 frames per call");
   if (cin < 3 || (!channels_last && cin != 3)) return set_error(SVR2_ERR_ARG, "svr2_resize: need >= 3 channels");
   const int K = taps_for(h, H) > taps_for(w, W) ? taps_for(h, H) : taps_for(w, W);
-  if (K > kMaxTaps) return set_error(SVR2_ERR_ARG, "svr2_resize: down-scale factor too large (> 7x)");
+  if (K > kMaxTaps) return set_error(SVR2_ERR_ARG, "svr2_resize: down-scale factor above 7.5 (more than 31 taps)");
   if (!scratch || scratch_bytes < svr2_resize_scratch_bytes(h, w, H, W))
     return set_error(SVR2_ERR_ARG, "svr2_resize: scratch too small (svr2_resize_scratch_bytes)");
   cudaStream_t s = (cudaStream_t)stream;

@@ -438,7 +438,16 @@ int svr2_ndhwc_to_ncdhw_seam_bf16(const void* in, int ld_in, int C, int T, int H
  * bf16(fp16(fp32(u) / 255)), the reference CLI's reading of 8-bit RGB frames (inference_cli.py:613, 336-339).
  *   finish == 0: out [T,3,H,W] bf16 (plain resize);
  *   finish != 0: out [3,T,Hp,Wp] bf16 = clamp(0,1) -> zero pad to multiples of 16 -> (x - 0.5) / 0.5 -> c t h w,
- *                Hp = ceil16(H), Wp = ceil16(W)  (what VideoDiffusionInfer.vae_encode consumes). */
+ *                Hp = ceil16(H), Wp = ceil16(W)  (what VideoDiffusionInfer.vae_encode consumes).
+ * The tap tables are torch's CUDA kernel's (upsample_antialias, fp32), so the result equals the reference's resize on
+ * the GPU bit for bit.  Down-scale factors above 7.5 per axis (more than 31 taps) are refused.
+ * Scratch: svr2_resize_scratch_bytes(h, w, H, W) bytes.  After a call it holds the tap tables, with L = max(H, W),
+ * K = the larger of the two axes' tap counts 2 ceil(2 max(in / out, 1)) + 1 (fp32 in / out), align256(n) = n rounded
+ * up to a multiple of 256:
+ *   offset 0:                          int32 xfirst[L], xcount[L]   (first input column and tap count per output column)
+ *   offset align256(8L):               int32 yfirst[L], ycount[L]   (the same per output row)
+ *   offset 2 align256(8L):             float xw[W][K]               (normalised weights; taps count..K-1 are 0)
+ *   offset 2 align256(8L) + align256(4LK): float yw[H][K]. */
 int64_t svr2_resize_scratch_bytes(int h, int w, int H, int W);
 int svr2_resize_bicubic_aa_bf16(const void* in, int in_dtype, int channels_last, int cin, int frames, int h, int w,
                                 void* out, int H, int W, int finish, void* scratch, int64_t scratch_bytes, void* stream);
@@ -456,7 +465,8 @@ int64_t svr2_alpha_upscale_scratch_bytes(int frames, int h, int w, int H, int W)
  *   rgb_up [frames,3,H,W] bf16: the decoded sample before colour correction, the guide (:331-337);
  *   binary mask = (count(a < 0.1) + count(a > 0.9)) / numel > 0.95 over all frames (:319-324);
  *   guide = (rgb + 1) / 2 when min(rgb) < 0; Sobel edges of the guide (detect_edges_batch, :125-188, bit-exact);
- *   base = antialiased bicubic resize of the alpha to H x W, clamp(0, 1) (:342-348);
+ *   base = antialiased bicubic resize of the alpha to H x W, clamp(0, 1) (:342-348), the tap tables and accumulation
+ *     of svr2_resize_bicubic_aa_bf16 (torch's CUDA kernel, bit for bit; down-scales up to 7.5 per axis);
  *   guided filter of base by mean(guide) (:191-286), radius 2 (binary) or 3, eps 0.002; binary masks then the
  *   edge-zone refinement of :370-408; clamp(0, 1).
  * out_kind 0: out [frames,H,W] fp32;  1: out [frames,H,W,4] bf16, channel 3 written (the RGBA image);

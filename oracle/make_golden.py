@@ -303,21 +303,26 @@ def pre_inputs(T, h, w, seed=3):
     return torch.rand(T, h, w, 3, generator=g) * 1.1 - 0.05     # [T,h,w,3], slightly outside [0,1]
 
 
-def run_pre_cases():
+def reference_compose(res, mx):
     """The reference's own transform classes composed as prepare_video_transforms does
-    (src/core/generation_utils.py:72-84), run on CPU on the bf16 clip (generation_phases.py:380-413)."""
+    (src/core/generation_utils.py:72-84)."""
     import importlib
     if ref_import.REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, ref_import.REFERENCE_ROOT)
     na = importlib.import_module("src.data.image.transforms.na_resize")
     dc = importlib.import_module("src.data.image.transforms.divisible_crop")
     from torchvision.transforms import Compose, Lambda, Normalize
+    return Compose([na.NaResize(resolution=res, mode="side", downsample_only=False, max_resolution=mx),
+                    Lambda(lambda x: torch.clamp(x, 0.0, 1.0)), dc.DivisiblePad((16, 16)), Normalize(0.5, 0.5),
+                    Lambda(lambda x: x.permute(1, 0, 2, 3))])
+
+
+def run_pre_cases():
+    """reference_compose run on CPU on the bf16 clip (generation_phases.py:380-413)."""
     from oracle import pre_oracle
 
     for name, (T, h, w, res, mx) in PRE_CASES.items():
-        tf = Compose([na.NaResize(resolution=res, mode="side", downsample_only=False, max_resolution=mx),
-                      Lambda(lambda x: torch.clamp(x, 0.0, 1.0)), dc.DivisiblePad((16, 16)), Normalize(0.5, 0.5),
-                      Lambda(lambda x: x.permute(1, 0, 2, 3))])
+        tf = reference_compose(res, mx)
         frames = pre_inputs(T, h, w)
         ref = tf(frames.to(torch.bfloat16).permute(0, 3, 1, 2))
         assert ref.dtype == torch.bfloat16

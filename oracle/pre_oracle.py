@@ -11,14 +11,18 @@ Third-party algorithm restated: torchvision 0.26 ``resize`` on a bf16 tensor cas
 ``torch.nn.functional.interpolate(mode="bicubic", align_corners=False, antialias=True)`` and casts the
 result back (``_functional_tensor.resize``); torch 2.11 ``_upsample_bicubic2d_aa`` = separable
 Keys cubic (a = -0.5) whose support widens by the down-scale factor, weights normalised to sum 1.
-Pinned: ``oracle/make_golden.py`` runs the reference's own transform classes on CPU and checks this
-restatement against them (``tests/golden/pre_*.npz``); the GPU tests additionally compare the kernel with
-torch's CUDA ``interpolate`` on the GPU.
+``aa_weights`` restates torch's CPU kernel, which made the goldens: ``oracle/make_golden.py`` runs the
+reference's own transform classes on the CPU and checks this restatement against them
+(``tests/golden/pre_*.npz``).  The reference runs its transform on the GPU, i.e. torch's CUDA kernel, whose
+fp32 tap arithmetic differs from the CPU kernel's in the last bits (csrc/aa_resize.cuh); the device kernel
+follows the CUDA one, and ``preprocess_torch`` below is the reference's op chain on any device, the bit-exact
+yardstick of tests/test_resize_elementwise_gpu.py.
 """
 from __future__ import annotations
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 
 def resized_size(h: int, w: int, resolution: int, max_resolution: int = 0):
@@ -99,3 +103,41 @@ def preprocess(frames: torch.Tensor, resolution: int, max_resolution: int = 0) -
     y = torch.nn.functional.pad(y, (0, pw, 0, ph))
     y = ((y - 0.5).to(torch.bfloat16).float() / 0.5).to(torch.bfloat16).float()
     return y.permute(1, 0, 2, 3).contiguous()
+
+
+# ---- the reference's op chain as torch ops, on the clip's own device
+def compute_dtype(x: torch.Tensor) -> torch.Tensor:
+    """A clip in the pipeline's bf16 compute dtype (generation_phases.py:380-388); 8-bit frames as the reference CLI
+    reads them, fp16(fp32(u) / 255) (inference_cli.py:613, 336-339), then bf16."""
+    if x.dtype == torch.uint8:
+        x = (x.float() / 255.0).half()
+    return x.to(torch.bfloat16)
+
+
+def resize_bf16(x: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """torchvision's resize of a bf16 [..., h, w] tensor: nothing at the same size, otherwise fp32,
+    interpolate(bicubic, align_corners=False, antialias=True), back to bf16."""
+    if tuple(x.shape[-2:]) == (H, W):
+        return x
+    return F.interpolate(x.float(), size=(H, W), mode="bicubic", align_corners=False, antialias=True).to(torch.bfloat16)
+
+
+def finish_bf16(y: torch.Tensor) -> torch.Tensor:
+    """[T, 3, H, W] bf16 -> [3, T, Hp, Wp]: clamp(0, 1), DivisiblePad((16, 16)) (zeros at the bottom / right),
+    Normalize(0.5, 0.5) in place in bf16, t c h w -> c t h w (a view, as the reference's Lambda returns it)."""
+    y = y.clamp(0.0, 1.0)
+    H, W = y.shape[-2:]
+    y = F.pad(y, (0, (16 - W % 16) % 16, 0, (16 - H % 16) % 16), mode="constant", value=0.0)
+    return y.sub_(0.5).div_(0.5).permute(1, 0, 2, 3)
+
+
+def preprocess_torch(clip_tchw: torch.Tensor, resolution: int, max_resolution: int = 0) -> torch.Tensor:
+    """prepare_video_transforms(resolution, max_resolution) on a [T, 3, h, w] clip in the compute dtype, as torch ops
+    on the clip's device: on a GPU tensor this is the reference's Compose exactly (torch's CUDA resize)."""
+    h, w = clip_tchw.shape[-2:]
+    (H, W), twice = resized_size(h, w, resolution, max_resolution)
+    x = clip_tchw
+    if twice:
+        (H1, W1), _ = resized_size(h, w, resolution, 0)
+        x = resize_bf16(x, H1, W1)
+    return finish_bf16(resize_bf16(x, H, W))

@@ -112,6 +112,23 @@ def test_pre_oracle_sizes_and_weights():
     assert np.allclose(np.sort(w, 1)[:, -1], 1.0) and np.allclose(np.abs(w).sum(1), 1.0)
 
 
+@pytest.mark.parametrize("T,h,w,res,mx", [(2, 30, 41, 90, 0), (2, 64, 48, 40, 0), (1, 36, 64, 108, 160),
+                                          (2, 33, 57, 33, 0), (1, 61, 23, 47, 0), (1, 45, 80, 72, 100)])
+def test_torch_op_chain_is_the_reference_compose(T, h, w, res, mx):
+    """pre_oracle.preprocess_torch, the yardstick the GPU resize is held to bit for bit on the device, is the
+    reference's own Compose (NaResize, clamp, DivisiblePad, Normalize, permute): bit-equal on the CPU, where both run
+    the same torch kernels, so that every cast, the second resize of the cap and the padding are the reference's."""
+    from oracle import make_golden, ref_import
+    if not os.path.isdir(os.path.join(ref_import.REFERENCE_ROOT, "src")):
+        pytest.skip("the reference sources are not installed")
+    g = torch.Generator().manual_seed(h * w + res)
+    clip = (torch.rand(T, 3, h, w, generator=g) * 1.2 - 0.1).to(torch.bfloat16)
+    ref = make_golden.reference_compose(res, mx)(clip.clone())
+    out = pre_oracle.preprocess_torch(clip.clone(), res, mx)
+    assert out.dtype == ref.dtype == torch.bfloat16 and out.shape == ref.shape
+    assert torch.equal(out, ref)
+
+
 def test_blend_overlap_oracle_matches_reference_golden(pkg):
     """blend_overlapping_frames (generation_utils.py:284-312): same inputs as oracle/make_golden.py, bit for bit;
     the host-side weight table of shard.py is the same computation."""

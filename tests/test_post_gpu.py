@@ -115,8 +115,9 @@ def _pre_cases():
 
 @pytest.mark.parametrize("name", list(_pre_cases()))
 def test_preprocess_vs_reference_golden(pre, name):
-    """prepare_video_transforms goldens: resize + clamp + pad-16 + normalise + c t h w in one kernel; equal up to one
-    bf16 ulp where the fp32 accumulation order flips a rounding."""
+    """prepare_video_transforms goldens: resize + clamp + pad-16 + normalise + c t h w in one kernel.  The goldens were
+    made on the CPU, whose tap arithmetic differs from that of torch's CUDA kernel (which the kernel follows, see
+    tests/test_resize_elementwise_gpu.py) in the last fp32 bits: equal up to one bf16 ulp where that flips a rounding."""
     from oracle.make_golden import pre_inputs
     T, h, w, res, mx = _pre_cases()[name]
     ref = torch.from_numpy(np.load(os.path.join(GOLD, name + ".npz"))["out"])
@@ -128,25 +129,6 @@ def test_preprocess_vs_reference_golden(pre, name):
     # the t c h w entry point (the reference's Compose is called on t c h w) gives the same result
     out2 = pre.prepare_video_transforms(res, mx)(frames.cuda().to(torch.bfloat16).permute(0, 3, 1, 2))
     assert torch.equal(out, out2)
-
-
-@pytest.mark.parametrize("h,w,H,W", [(180, 320, 540, 960), (270, 480, 1080, 1920), (200, 300, 150, 225)])
-def test_resize_matches_torch_cuda_interpolate(svr2lib, h, w, H, W):
-    """The resize alone against torch's own CUDA kernel (what torchvision's resize runs on a GPU tensor):
-    interpolate(fp32(bf16 clip), bicubic, antialias=True) -> bf16."""
-    g = torch.Generator().manual_seed(9)
-    x = torch.rand(2, 3, h, w, generator=g).to(torch.bfloat16).cuda()
-    ref = torch.nn.functional.interpolate(x.float(), size=(H, W), mode="bicubic", align_corners=False,
-                                          antialias=True).to(torch.bfloat16)
-    out = torch.empty(2, 3, H, W, device="cuda", dtype=torch.bfloat16)
-    need = svr2lib.load().svr2_resize_scratch_bytes(h, w, H, W)
-    scratch = torch.empty(need, device="cuda", dtype=torch.uint8)
-    svr2lib.call("svr2_resize_bicubic_aa_bf16", svr2lib.ptr(x), 1, 0, 3, 2, h, w, svr2lib.ptr(out), H, W, 0,
-                 svr2lib.ptr(scratch), need, svr2lib.stream())
-    # fp32 rounding of the tap weights / accumulation differs in the last bit, which flips the final bf16 rounding
-    # of about one output in a thousand by one ulp
-    d = (out.float() - ref.float()).abs()
-    assert (d == 0).float().mean() > 0.995 and d.max() <= 2 ** -7, ((d == 0).float().mean().item(), d.max().item())
 
 
 def test_preprocess_identity_size_and_padding(pre):
