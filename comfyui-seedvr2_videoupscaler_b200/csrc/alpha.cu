@@ -55,16 +55,20 @@ __device__ __forceinline__ int reflect101(int i, int n) {
   return i < 0 ? 0 : (i >= n ? n - 1 : i);
 }
 
-// Guide value of one channel and the grayscale guide I = mean over RGB (torch's CPU mean: sum, then / 3)
-__device__ __forceinline__ float guide_gray(const __nv_bfloat16* px, long long plane, int norm) {
+// Guide value of one channel and the grayscale guide I = guide.mean(dim=1) as torch's CUDA reduction computes it on the
+// reference's GPU tensor: the channel sum in order, then MeanOps' multiply by its fp32 factor (guide_factor)
+__device__ __forceinline__ float guide_gray(const __nv_bfloat16* px, long long plane, int norm, float factor) {
   float c[3];
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     const float v = bf(px + k * plane);
     c[k] = norm ? half01(v) : v;
   }
-  return __fdiv_rn(__fadd_rn(__fadd_rn(c[0], c[1]), c[2]), 3.f);
+  return __fmul_rn(__fadd_rn(__fadd_rn(c[0], c[1]), c[2]), factor);
 }
+
+// ATen's mean factor, float(outputs) / numel with numel converted to float: fl(1/3) unless 3 T H W rounds in fp32
+inline float guide_factor(long long outputs) { return (float)outputs / (float)(3 * outputs); }
 
 // cv2.cvtColor(RGB2GRAY) of the uint8 image made by detect_edges_batch (:148-159)
 __device__ __forceinline__ int gray_u8(const __nv_bfloat16* px, long long plane, int norm, int twice) {
@@ -123,15 +127,16 @@ __global__ void __launch_bounds__(256) alpha_stats_kernel(const T* __restrict__ 
   }
 }
 
-// The flags, in the reference's fp32 order: (near_zero.float() + near_one.float()) / numel > 0.95
+// The flags, in the reference's fp32 order: (near_zero.float() + near_one.float()) / numel > 0.95, the division by
+// the Python int numel as torch's CUDA kernel does it: a multiply by fl(1 / fl(numel)) (div_true_kernel_cuda)
 __global__ void alpha_finalize_kernel(AlphaHdr* __restrict__ hdr, long long n_alpha, int allow_twice) {
   const float m = key_min(hdr->min_key);
   const int norm = m < 0.f;
   hdr->rgb_min = m;
   hdr->normalise = norm;
   hdr->normalise_twice = allow_twice && norm && half01(m) < 0.f;
-  const float ratio = n_alpha > 0 ? __fdiv_rn(__fadd_rn(__ull2float_rn(hdr->n_low), __ull2float_rn(hdr->n_high)),
-                                              __ll2float_rn(n_alpha))
+  const float ratio = n_alpha > 0 ? __fmul_rn(__fadd_rn(__ull2float_rn(hdr->n_low), __ull2float_rn(hdr->n_high)),
+                                              __frcp_rn(__ll2float_rn(n_alpha)))
                                   : 0.f;
   hdr->ratio = ratio;
   hdr->binary = ratio > 0.95f;
@@ -231,12 +236,13 @@ __device__ __forceinline__ float box_mean(const float* __restrict__ c) {
 template <int R>
 __device__ __forceinline__ void guided_a(float* __restrict__ sI, float* __restrict__ sP,
                                          const __nv_bfloat16* __restrict__ img, const float* __restrict__ p,
-                                         float* __restrict__ A, float* __restrict__ B, int H, int W, int norm) {
+                                         float* __restrict__ A, float* __restrict__ B, int H, int W, int norm,
+                                         float factor) {
   constexpr int TW = kTile + 2 * R;
   constexpr float K = (float)((2 * R + 1) * (2 * R + 1));
   const int x0 = blockIdx.x * kTile, y0 = blockIdx.y * kTile;
   const long long plane = (long long)H * W;
-  load_tile<R>(sI, x0, y0, H, W, [&](int y, int x) { return guide_gray(img + (long long)y * W + x, plane, norm); });
+  load_tile<R>(sI, x0, y0, H, W, [&](int y, int x) { return guide_gray(img + (long long)y * W + x, plane, norm, factor); });
   load_tile<R>(sP, x0, y0, H, W, [&](int y, int x) { return p[(long long)y * W + x]; });
   __syncthreads();
   const int tx = threadIdx.x & 31;
@@ -269,14 +275,14 @@ __device__ __forceinline__ void guided_a(float* __restrict__ sI, float* __restri
 // Pass A: one frame per blockIdx.z; the radius comes from the statistics (uniform per launch).
 __global__ void __launch_bounds__(256) guided_a_kernel(const __nv_bfloat16* __restrict__ rgb, const float* __restrict__ p,
                                                        float* __restrict__ A, float* __restrict__ B, int H, int W,
-                                                       const AlphaHdr* __restrict__ hdr) {
+                                                       float factor, const AlphaHdr* __restrict__ hdr) {
   __shared__ float sI[(kTile + 6) * (kTile + 6)], sP[(kTile + 6) * (kTile + 6)];
   const long long plane = (long long)H * W, t = blockIdx.z;
   const int norm = hdr->normalise;
   if (hdr->radius == 2)
-    guided_a<2>(sI, sP, rgb + t * 3 * plane, p + t * plane, A + t * plane, B + t * plane, H, W, norm);
+    guided_a<2>(sI, sP, rgb + t * 3 * plane, p + t * plane, A + t * plane, B + t * plane, H, W, norm, factor);
   else
-    guided_a<3>(sI, sP, rgb + t * 3 * plane, p + t * plane, A + t * plane, B + t * plane, H, W, norm);
+    guided_a<3>(sI, sP, rgb + t * 3 * plane, p + t * plane, A + t * plane, B + t * plane, H, W, norm, factor);
 }
 
 // Steps 3-8 of the binary-mask branch (:370-408) for one pixel: q is the guided-filter output, e the edge value and z
@@ -296,7 +302,7 @@ template <int R, bool BIN>
 __device__ __forceinline__ void guided_b(float* __restrict__ sA, float* __restrict__ sB, unsigned* __restrict__ sS,
                                          const __nv_bfloat16* __restrict__ img, const float* __restrict__ A,
                                          const float* __restrict__ B, const unsigned* __restrict__ sq, unsigned smax,
-                                         int H, int W, int norm, int t, float* __restrict__ out_f32,
+                                         int H, int W, int norm, float factor, int t, float* __restrict__ out_f32,
                                          __nv_bfloat16* __restrict__ out_rgba) {
   constexpr int TW = kTile + 2 * R, SW = kTile + 2;
   const int x0 = blockIdx.x * kTile, y0 = blockIdx.y * kTile;
@@ -316,7 +322,7 @@ __device__ __forceinline__ void guided_b(float* __restrict__ sA, float* __restri
     if (y >= H || x >= W) continue;
     const long long o = (long long)y * W + x;
     const float ma = box_mean<R>(sA + ty * TW + tx), mb = box_mean<R>(sB + ty * TW + tx);
-    float v = __fadd_rn(__fmul_rn(ma, guide_gray(img + o, plane, norm)), mb);
+    float v = __fadd_rn(__fmul_rn(ma, guide_gray(img + o, plane, norm, factor)), mb);
     if (BIN) {
       const unsigned* c = sS + (ty + 1) * SW + tx + 1;
       unsigned zmax = 0;
@@ -337,7 +343,8 @@ __device__ __forceinline__ void guided_b(float* __restrict__ sA, float* __restri
 __global__ void __launch_bounds__(256) guided_b_kernel(const __nv_bfloat16* __restrict__ rgb, const float* __restrict__ A,
                                                        const float* __restrict__ B, const unsigned* __restrict__ sq,
                                                        const unsigned* __restrict__ frame_max, int H, int W,
-                                                       const AlphaHdr* __restrict__ hdr, float* __restrict__ out_f32,
+                                                       float factor, const AlphaHdr* __restrict__ hdr,
+                                                       float* __restrict__ out_f32,
                                                        __nv_bfloat16* __restrict__ out_rgba) {
   __shared__ float sA[(kTile + 6) * (kTile + 6)], sB[(kTile + 6) * (kTile + 6)];
   __shared__ unsigned sS[(kTile + 2) * (kTile + 2)];
@@ -345,11 +352,11 @@ __global__ void __launch_bounds__(256) guided_b_kernel(const __nv_bfloat16* __re
   const int t = blockIdx.z, norm = hdr->normalise;
   const __nv_bfloat16* img = rgb + (long long)t * 3 * plane;
   if (hdr->binary)
-    guided_b<2, true>(sA, sB, sS, img, A + t * plane, B + t * plane, sq + t * plane, frame_max[t], H, W, norm, t,
-                      out_f32, out_rgba);
+    guided_b<2, true>(sA, sB, sS, img, A + t * plane, B + t * plane, sq + t * plane, frame_max[t], H, W, norm, factor,
+                      t, out_f32, out_rgba);
   else
-    guided_b<3, false>(sA, sB, sS, img, A + t * plane, B + t * plane, sq + t * plane, 0u, H, W, norm, t, out_f32,
-                       out_rgba);
+    guided_b<3, false>(sA, sB, sS, img, A + t * plane, B + t * plane, sq + t * plane, 0u, H, W, norm, factor, t,
+                       out_f32, out_rgba);
 }
 
 // [T,3,hw] -> channels 0..2 of [T,hw,4]: clamp(-1,1) * 0.5 + 0.5 with the rounding of sample_to_image (post.cu);
@@ -475,8 +482,9 @@ extern "C" int svr2_alpha_upscale(const void* alpha_src, int src_dtype, int src_
   const dim3 tgrid((W + kTile - 1) / kTile, (H + kTile - 1) / kTile, frames);
   const __nv_bfloat16* rgb = (const __nv_bfloat16*)rgb_up;
   sobel_sq_kernel<<<tgrid, 256, 0, s>>>(rgb, H, W, sq, fmax, hdr);
-  guided_a_kernel<<<tgrid, 256, 0, s>>>(rgb, p, A, B, H, W, hdr);
-  guided_b_kernel<<<tgrid, 256, 0, s>>>(rgb, A, B, sq, fmax, H, W, hdr, out_kind == 0 ? (float*)out : nullptr,
+  const float factor = guide_factor((long long)frames * plane);
+  guided_a_kernel<<<tgrid, 256, 0, s>>>(rgb, p, A, B, H, W, factor, hdr);
+  guided_b_kernel<<<tgrid, 256, 0, s>>>(rgb, A, B, sq, fmax, H, W, factor, hdr, out_kind == 0 ? (float*)out : nullptr,
                                         out_kind == 1 ? (__nv_bfloat16*)out : nullptr);
   return check_launch("alpha_guided_filter");
 }

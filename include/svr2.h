@@ -456,18 +456,28 @@ int svr2_resize_bicubic_aa_bf16(const void* in, int in_dtype, int channels_last,
  * generation_phases.py:1142-1217).  All in fp32, no host synchronisation.
  * Scratch: svr2_alpha_upscale_scratch_bytes(frames, h, w, H, W) bytes.  After a call its first 24 bytes hold
  *   int32 binary, normalise, normalise_twice, radius; float32 binary_ratio, guide_min
- * (the branch decisions of :319-334 and of detect_edges_batch :148-149, which the later kernels read on the device). */
+ * (the branch decisions of :319-334 and of detect_edges_batch :148-149, which the later kernels read on the device).
+ * The rest of the scratch, n = frames H W, L = max(H, W), K = the resize's taps per output (svr2_resize_scratch_bytes):
+ *   offset 24: 24 bytes of working state (the running minimum's key, the two counts);
+ *   offset 48: uint32 frame_max[frames], each frame's max of gx^2 + gy^2;
+ *   offset S = align256(48 + 4 frames): uint32 gx^2 + gy^2 [frames,H,W];
+ *   offset S + align256(4n): the resize tap tables, laid out as in svr2_resize_scratch_bytes, 2 align256(8L) +
+ *     2 align256(4LK) bytes;
+ *   then three fp32 [frames,H,W] planes, each align256(4n) bytes apart: p (the clamped base), a and b (pass A).
+ * A NaN in the guide is skipped by its minimum (fminf), where torch's min() would return NaN. */
 int64_t svr2_alpha_upscale_scratch_bytes(int frames, int h, int w, int H, int W);
 /* Steps of :310-426 for `frames` frames:
  *   alpha_src [frames,h,w,src_channels] (src_channels 4: RGBA frames, 1: an alpha plane), the alpha is the last
  *     channel; src_dtype 0 fp32 | 1 bf16 | 2 fp16 | 3 uint8 (loaded as the resize loads it), rounded to bf16 on load
  *     (the clip in the compute dtype, :407-473);
  *   rgb_up [frames,3,H,W] bf16: the decoded sample before colour correction, the guide (:331-337);
- *   binary mask = (count(a < 0.1) + count(a > 0.9)) / numel > 0.95 over all frames (:319-324);
+ *   binary mask = (count(a < 0.1) + count(a > 0.9)) / numel > 0.95 over all frames (:319-324), the counts and numel
+ *     rounded to fp32 and the division a multiply by fl(1 / numel) (torch's CUDA tensor / scalar);
  *   guide = (rgb + 1) / 2 when min(rgb) < 0; Sobel edges of the guide (detect_edges_batch, :125-188, bit-exact);
  *   base = antialiased bicubic resize of the alpha to H x W, clamp(0, 1) (:342-348), the tap tables and accumulation
  *     of svr2_resize_bicubic_aa_bf16 (torch's CUDA kernel, bit for bit; down-scales up to 7.5 per axis);
- *   guided filter of base by mean(guide) (:191-286), radius 2 (binary) or 3, eps 0.002; binary masks then the
+ *   guided filter of base by the guide's channel mean (:191-286) rounded as torch's CUDA mean: fl(fl(c0 + c1) + c2)
+ *     times fl(fl(frames H W) / fl(3 frames H W)), radius 2 (binary) or 3, eps 0.002; binary masks then the
  *   edge-zone refinement of :370-408; clamp(0, 1).
  * out_kind 0: out [frames,H,W] fp32;  1: out [frames,H,W,4] bf16, channel 3 written (the RGBA image);
  *          2: out [frames,H,W] fp32 = the clamped base resize alone (inspection of that step). */

@@ -15,9 +15,12 @@ EPS = 0.002
 
 
 def binary_ratio(alpha: torch.Tensor):
-    """(near_zero.float() + near_one.float()) / numel and ratio > 0.95 (:319-324)."""
+    """(near_zero.float() + near_one.float()) / numel and ratio > 0.95 (:319-324), the reference's ops literally: a
+    true division on the CPU, a multiply by fl(1 / fl(numel)) on the GPU."""
     flat = alpha.float().flatten()
-    ratio = ((flat < 0.1).sum().float() + (flat > 0.9).sum().float()) / flat.numel()
+    near_zero = (flat < 0.1).sum().float()
+    near_one = (flat > 0.9).sum().float()
+    ratio = (near_zero + near_one) / flat.numel()
     return ratio, bool(ratio > 0.95)
 
 
@@ -27,10 +30,17 @@ def gray_u8(u8: torch.Tensor) -> torch.Tensor:
     return (9798 * u[:, 0] + 19235 * u[:, 1] + 3735 * u[:, 2] + (1 << 14)) >> 15
 
 
+def reflect101(n: int, device) -> torch.Tensor:
+    """Indices -1..n of an axis of length n under OpenCV's BORDER_REFLECT_101 (a one-pixel axis reflects onto itself)."""
+    i = torch.arange(-1, n + 1, device=device).abs()
+    return torch.where(i >= n, 2 * n - 2 - i, i).clamp(0, n - 1)
+
+
 def sobel_sq(gray: torch.Tensor) -> torch.Tensor:
-    """gx^2 + gy^2 of cv2.Sobel(gray, CV_64F, 1,0 / 0,1, ksize=3), BORDER_REFLECT_101 (torch 'reflect'), fp64 (exact
-    integers).  gray (T,H,W) with H, W >= 2."""
-    p = F.pad(gray.to(torch.float64)[:, None], (1, 1, 1, 1), mode="reflect")[:, 0]
+    """gx^2 + gy^2 of cv2.Sobel(gray, CV_64F, 1,0 / 0,1, ksize=3), BORDER_REFLECT_101, fp64 (exact integers).  gray
+    (T,H,W), any H, W >= 1 (torch's 'reflect' pad needs 2)."""
+    H, W = gray.shape[1:]
+    p = gray.to(torch.float64)[:, reflect101(H, gray.device)][:, :, reflect101(W, gray.device)]
     gx = (p[:, :-2, 2:] - p[:, :-2, :-2]) + 2 * (p[:, 1:-1, 2:] - p[:, 1:-1, :-2]) + (p[:, 2:, 2:] - p[:, 2:, :-2])
     gy = (p[:, 2:, :-2] - p[:, :-2, :-2]) + 2 * (p[:, 2:, 1:-1] - p[:, :-2, 1:-1]) + (p[:, 2:, 2:] - p[:, :-2, 2:])
     return gx * gx + gy * gy
@@ -54,14 +64,27 @@ def box(x: torch.Tensor, r: int) -> torch.Tensor:
     return F.avg_pool2d(x, kernel_size=2 * r + 1, stride=1, padding=r)
 
 
-def guided_filter(I: torch.Tensor, p: torch.Tensor, r: int, eps: float = EPS) -> torch.Tensor:
-    """_apply_guided_filter (:234-286)."""
+def guided_filter(I: torch.Tensor, p: torch.Tensor, r: int, eps: float = EPS, taps: dict = None) -> torch.Tensor:
+    """_apply_guided_filter (:234-286); taps receives the coefficients a and b."""
     mI, mp = box(I, r), box(p, r)
     var = box(I * I, r) - mI * mI
     cov = box(I * p, r) - mI * mp
     a = cov / (var + eps)
     b = mp - a * mI
+    if taps is not None:
+        taps.update(a=a, b=b)
     return box(a, r) * I + box(b, r)
+
+
+def refine_binary(q: torch.Tensor, edges: torch.Tensor, taps: dict) -> torch.Tensor:
+    """Steps 3-8 of the binary-mask branch (:370-408) on the guided filter's output q."""
+    zone = F.max_pool2d(edges, kernel_size=3, stride=1, padding=1)
+    in_edges = q * (1 - torch.clamp(edges / 0.25, 0, 1)) + torch.sigmoid((q - 0.5) * 12.0) * torch.clamp(edges / 0.25, 0, 1)
+    combined = torch.where(zone < 0.05, (q > 0.5).float(), in_edges)
+    pre = torch.where(zone < 0.03, (combined > 0.5).float(), combined)
+    out = torch.where((pre > 0.3) & (pre < 0.7) & ~(edges > 0.15), (pre > 0.5).float(), pre)
+    taps.update(q=q, zone=zone, combined=combined, pre_cleanup=pre)
+    return out
 
 
 def edge_guided_alpha_upscale(input_alpha: torch.Tensor, upscaled_rgb: torch.Tensor, taps: dict = None) -> torch.Tensor:
@@ -76,20 +99,14 @@ def edge_guided_alpha_upscale(input_alpha: torch.Tensor, upscaled_rgb: torch.Ten
     taps["normalise_twice"] = bool(rgb_n.min() < 0)
     edges = detect_edges_batch(rgb_n)
     base = F.interpolate(alpha, size=(H, W), mode="bicubic", align_corners=False, antialias=True).clamp(0, 1)
-    # guide.mean(dim=1) as the reference's CPU run computes it: the channel sum, then a true division by 3
-    I = (rgb_n[:, 0:1] + rgb_n[:, 1:2]) + rgb_n[:, 2:3]
-    I = I / torch.full_like(I, 3.0)
-    taps.update(edges=edges, base=base)
+    # guide.mean(dim=1) (:212): on the CPU the channel sum over 3; on the GPU the sum times ATen's fp32 mean factor
+    I = rgb_n.mean(dim=1, keepdim=True)
+    taps.update(edges=edges, base=base, guide=I)
     if is_binary:
-        q = guided_filter(I, base, 2)
-        zone = F.max_pool2d(edges, kernel_size=3, stride=1, padding=1)
-        in_edges = q * (1 - torch.clamp(edges / 0.25, 0, 1)) + torch.sigmoid((q - 0.5) * 12.0) * torch.clamp(edges / 0.25, 0, 1)
-        combined = torch.where(zone < 0.05, (q > 0.5).float(), in_edges)
-        pre = torch.where(zone < 0.03, (combined > 0.5).float(), combined)
-        out = torch.where((pre > 0.3) & (pre < 0.7) & ~(edges > 0.15), (pre > 0.5).float(), pre)
-        taps.update(q=q, zone=zone, combined=combined, pre_cleanup=pre)
+        q = guided_filter(I, base, 2, taps=taps)
+        out = refine_binary(q, edges, taps)
     else:
-        q = guided_filter(I, base, 3)
+        q = guided_filter(I, base, 3, taps=taps)
         out = q
         taps.update(q=q)
     return out.clamp(0, 1)

@@ -31,7 +31,11 @@ def run_kind(am, src, channels, rgb, kind):
 
 
 def check_against(out, ref, taps, binary, tag):
-    """Gradient alphas: max |d| <= 1e-4, bf16 casts >= 99.5 % equal and otherwise one bf16 ulp apart (the ulp taken at
+    """Against the goldens, which the reference made on the CPU.  The kernel follows torch's CUDA rounding, as the
+    reference does on its GPU tensors: the guide's mean is the channel sum times an fp32 factor there and a true
+    division by 3 on the CPU, and the CPU's box sums need not add in the same order.  Those roundings move fp32 alphas
+    by a few 1e-6 and flip a binary-mask threshold where q sits that close to it, hence bounds this loose; the exact
+    checks are tests/test_alpha_elementwise_gpu.py and test_full_path_at_4k_vs_gpu_oracle.  Gradient alphas: max |d| <= 1e-4, bf16 casts >= 99.5 % equal and otherwise one bf16 ulp apart (the ulp taken at
     no less than 2^-8: below that, fp32 noise of 1e-9 is already several bf16 ulps of an invisible alpha).  Binary masks:
     <= 0.1 % of the pixels differ by more than 1e-4, each one where the oracle sat within 1e-4 of a threshold."""
     out, ref = out.float().cpu().reshape(ref.shape), ref.float().cpu()
@@ -61,25 +65,6 @@ def test_sobel_edges_bit_exact_at_4k(am):
     base = F.interpolate(torch.rand(2, 3, 68, 120, generator=g, device="cuda"), size=(2160, 3840), mode="bicubic")
     rgb = (base * 2.2 - 1.1 + 0.05 * torch.randn(2, 3, 2160, 3840, generator=g, device="cuda")).to(torch.bfloat16)
     assert torch.equal(am.detect_edges_batch(rgb), ao.detect_edges_batch(rgb))
-
-
-def test_statistics_flags_exact(am, svr2lib):
-    rgb = torch.full((1, 3, 40, 60), 0.25, device="cuda", dtype=torch.bfloat16)
-    # ratio exactly 0.95: not a binary mask (strict >), the ratio in fp32 as the reference computes it
-    a = torch.ones(1, 20, 40, 1)
-    a.view(-1)[torch.randperm(800, generator=torch.Generator().manual_seed(0))[:40]] = 0.5
-    f = am.read_flags(run_kind(am, a.cuda(), 1, rgb, am.OUT_RESIZE)[1])
-    assert f["binary"] is False and f["radius"] == 3 and f["binary_ratio"] == np.float32(0.95)
-    a.view(-1)[torch.nonzero(a.view(-1) == 0.5)[0]] = 0.05                 # 761 / 800 > 0.95
-    f = am.read_flags(run_kind(am, a.cuda(), 1, rgb, am.OUT_RESIZE)[1])
-    assert f["binary"] is True and f["radius"] == 2 and f["binary_ratio"] == np.float32(761) / np.float32(800)
-    # the guide's min: exactly 0 (no normalisation), -1e-7 (normalise once), below -1 (the edge detector normalises again)
-    for low, norm, twice in ((0.0, False, False), (-1e-7, True, False), (-1.5, True, True)):
-        g = rgb.clone()
-        g[0, 1, 7, 11] = low
-        f = am.read_flags(run_kind(am, a.cuda(), 1, g, am.OUT_RESIZE)[1])
-        assert (f["normalise"], f["normalise_twice"]) == (norm, twice), low
-        assert f["guide_min"] == torch.tensor(low).to(torch.bfloat16).item()
 
 
 @pytest.mark.parametrize("shape", [(2, 37, 53, 90, 128), (1, 90, 128, 37, 53), (3, 72, 128, 216, 384),
@@ -116,14 +101,15 @@ def test_full_path_vs_reference_goldens(am, name):
 
 @pytest.mark.parametrize("kind", ["binary", "gradient"])
 def test_full_path_at_4k_vs_gpu_oracle(am, kind):
-    """The 4K shard shape: 5 frames, 720p alpha -> 2160 x 3840."""
+    """The 4K shard shape: 5 frames, 720p alpha -> 2160 x 3840, bit for bit against the reference's op chain run by
+    torch on the GPU, as the reference runs it."""
     alpha, rgb = ao.make_inputs(5, 720, 1280, 2160, 3840, kind, seed=11)
     alpha, rgb = alpha.cuda(), rgb.cuda()
     out = am.edge_guided_alpha_upscale(alpha, None, rgb)
     taps = {}
     ref = ao.edge_guided_alpha_upscale(alpha, rgb, taps)
     assert taps["binary"] == (kind == "binary")
-    check_against(out, ref, taps, taps["binary"], kind)
+    assert torch.equal(out, ref), (kind, int((out != ref).sum()))
 
 
 # ---- the engine with synthetic weights
