@@ -421,28 +421,52 @@ class B200VideoVAE(EngineModule):
         y = self._gn(x, p + "group_norm", False, 0)
         yf = y.buf.view(x.T * n, C)
         q = lib.linear(yf, self.W[p + "to_q.weight"], bias=self.W[p + "to_q.bias"])
-        ldn = (n + 7) // 8 * 8
         # K carries 8 spare rows: pass 2 runs with N rounded up to a multiple of 8 (16-byte stores);
         # the extra score columns are never read by the P @ V GEMM (its K extent is n)
         k_buf = torch.empty(x.T * n + 8, C, device=dev, dtype=torch.bfloat16)
         k_buf[x.T * n:].zero_()
-        k_ = lib.linear(yf, self.W[p + "to_k.weight"], bias=self.W[p + "to_k.bias"], out=k_buf[: x.T * n])
+        lib.linear(yf, self.W[p + "to_k.weight"], bias=self.W[p + "to_k.bias"], out=k_buf[: x.T * n])
         v = lib.linear(yf, self.W[p + "to_v.weight"], bias=self.W[p + "to_v.bias"])
         del y, yf
+        o = self._softmax_v(q, k_buf, v, x.T, n, single_pass)
+        out = Act(x.T, x.H, x.W, C, 0, dev)
+        xb = x.body.reshape(x.T * n, C)
+        lib.linear(o, self.W[p + "to_out.0.weight"], bias=self.W[p + "to_out.0.bias"], residual=xb,
+                   out=out.buf.view(x.T * n, C))
+        return out
+
+    @staticmethod
+    def _attention_chunk_rows(n: int) -> int:
+        """Query rows per chunk of _softmax_v (vae_engine.cu attention computes the same): whole waves of m-tiles, as many
+        as keep the chunk's bf16 P under 4 GiB, never more rows than the frame's m-tiles hold."""
+        ldn = (n + 7) // 8 * 8
+        wave_rows = 66 * 128                       # 66 m-tiles x 2 n-tiles (d = 512) = one full wave of 132 CTAs
+        k = max(1, (1 << 32) // (wave_rows * ldn * 2))
+        return min(wave_rows * k, (n + 127) // 128 * 128)
+
+    def _softmax_v(self, q, k_buf, v, T: int, n: int, single_pass: bool = True, *, o=None, vt=None, P=None,
+                   flag_log=None):
+        """softmax(q k^T / sqrt(C)) v per frame for T frames of n tokens: q, v (T n, C); k_buf (T n + 8, C) whose last 8
+        rows are zero.  Returns o (T n, C) bf16.  Tests may pass the output `o`, the scratch `vt` (C, >= ceil8(n)) and
+        `P` (>= min(cq, n) rows, ldn columns) to guard them, and `flag_log` (int32, one entry per frame and query chunk) to
+        receive the single-pass fallback flag as each chunk's svr2_pexp_stat_combine left it."""
+        C, dev = q.shape[1], self.device
         # Two GEMM passes per query chunk, never materialising the fp32 score matrix:
         #   pass 1: per-row (max, sum exp2) partials of q k^T * scale  -> log2-sum-exp per row
         #   pass 2: P = bf16(exp2(q k^T * scale - lse))  (normalised probabilities)
         #   then   O = P @ V  (V consumed through its transpose, K-major)
         ldn = (n + 7) // 8 * 8
-        wave_rows = 66 * 128                       # 66 m-tiles x 2 n-tiles (d = 512) = one full wave of 132 CTAs
-        k = max(1, (1 << 32) // (wave_rows * ldn * 2))
-        cq = min(wave_rows * k, (n + 127) // 128 * 128)
+        cq = self._attention_chunk_rows(n)
         slots = lib.load().svr2_rowstat_slots(n)
-        vt = torch.empty(C, ldn, device=dev, dtype=torch.bfloat16)
+        if vt is None:
+            vt = torch.empty(C, ldn, device=dev, dtype=torch.bfloat16)
         part = torch.empty(min(cq, n), 2 * slots, device=dev, dtype=torch.float32)
         lse = torch.empty(min(cq, n), device=dev, dtype=torch.float32)
-        P = torch.empty(min(cq, n), ldn, device=dev, dtype=torch.bfloat16)
-        o = torch.empty(x.T * n, C, device=dev, dtype=torch.bfloat16)
+        if P is None:
+            P = torch.empty(min(cq, n), ldn, device=dev, dtype=torch.bfloat16)
+        if o is None:
+            o = torch.empty(T * n, C, device=dev, dtype=torch.bfloat16)
+        k_ = k_buf[:T * n]
         scale2 = (1.0 / (C ** 0.5)) * 1.4426950408889634
         # Default (n >= 256, n % 8 == 0): ONE Q K^T pass.  A 1/16-cost GEMM over every 16th key yields a reference
         # exponent per row; the full pass writes un-normalised bf16(exp2(s - ref)) and fp32 row sums; P~ @ V is divided
@@ -461,9 +485,9 @@ class B200VideoVAE(EngineModule):
             mhat = torch.empty(rows_max, device=dev, dtype=torch.float32)
             rscale = torch.empty(rows_max, device=dev, dtype=torch.float32)
             flag = torch.zeros(1, device=dev, dtype=torch.int32)
-        for f in range(x.T):
+        for f in range(T):
             qf, kf, vf = q[f * n:(f + 1) * n], k_[f * n:(f + 1) * n], v[f * n:(f + 1) * n]
-            lib.call("svr2_transpose_bf16", lib.ptr(vf), C, lib.ptr(vt), ldn, n, C, lib.stream())
+            lib.call("svr2_transpose_bf16", lib.ptr(vf), C, lib.ptr(vt), vt.stride(0), n, C, lib.stream())
             for r0 in range(0, n, cq):
                 rows = min(cq, n - r0)
                 qc, oc = qf[r0:r0 + rows], o[f * n + r0: f * n + r0 + rows]
@@ -473,6 +497,8 @@ class B200VideoVAE(EngineModule):
                     lib.linear(qc, kf, epi=lib.EPI_PEXP, gate=mhat, out=P[:rows], out_scale=scale2, stat_out=stat[:rows])
                     lib.call("svr2_pexp_stat_combine", lib.ptr(stat), slots_p, slots_p, lib.ptr(mhat), lib.ptr(rscale), rows,
                              lib.ptr(flag), lib.stream())
+                    if flag_log is not None:
+                        flag_log[f * -(-n // cq) + r0 // cq].copy_(flag[0])
                     lib.linear(P[:rows, :n], vt[:, :n], out=oc, rowscale=rscale)
                 run_if = flag if single else None        # exact path: unconditional, or the device-side fallback
                 lib.linear(qc, kf, epi=lib.EPI_ROWSTAT, out=part[:rows], out_scale=scale2, count_flops=False, run_if=run_if)
@@ -480,11 +506,7 @@ class B200VideoVAE(EngineModule):
                 lib.linear(qc, k_buf[f * n: f * n + ldn], epi=lib.EPI_PEXP, gate=lse, out=P[:rows], out_scale=scale2,
                            run_if=run_if, count_flops=not single)
                 lib.linear(P[:rows, :n], vt[:, :n], out=oc, run_if=run_if, count_flops=not single)
-        out = Act(x.T, x.H, x.W, C, 0, dev)
-        xb = x.body.reshape(x.T * n, C)
-        lib.linear(o, self.W[p + "to_out.0.weight"], bias=self.W[p + "to_out.0.bias"], residual=xb,
-                   out=out.buf.view(x.T * n, C))
-        return out
+        return o
 
     def _mid(self, x: Act, p: str) -> Act:
         x = self._resnet(x, p + "resnets.0.")

@@ -131,12 +131,16 @@ OK_EDGES = (f32(1e-30, INF), f32(1e30, 0.0), 1.0)      # the fp32 neighbours of 
 BAD_SUMS = (0.0, -0.0, f32(1e-30), 1e-40, -1.0, f32(1e30), 3e38, INF, -INF, NAN)
 
 
-@pytest.mark.parametrize("slots", [1, 6, 33, 70])
+# 254 / 1014: the row-sum slots of the 1080p and 4K latents (n = 32 400, 129 600), at a tail chunk's and a full chunk's rows
+PEXP_ROWS = {254: 2880, 1014: 8448}
+
+
+@pytest.mark.parametrize("slots", [1, 6, 33, 70, 254, 1014])
 def test_pexp_stat_combine_rowscale_and_flag(svr2lib, slots):
     """rowscale = 1 / (sum of the slots' .y) when it lies in (1e-30, 1e30), else 0 and the flag goes up; the flag is
     raised for sums <= 1e-30, >= 1e30, +-inf and NaN, and for no other sum.  203 rows (not a multiple of the 8 rows per
     block), slots past the 32 lanes, ld = slots + 2 with NaN in the spare slots and NaN in every .x (neither is read)."""
-    rows, ld = 203, slots + 2
+    rows, ld = PEXP_ROWS.get(slots, 203), slots + 2
     g = torch.Generator(device="cpu").manual_seed(slots)
     part = torch.full((rows, ld, 2), NAN)
     scale = 10.0 ** (torch.rand(rows, 1, generator=g) * 50 - 25)          # row sums from ~1e-25 to ~1e25
@@ -150,8 +154,9 @@ def test_pexp_stat_combine_rowscale_and_flag(svr2lib, slots):
     flag = _flag(0)
     base = _combine(svr2lib, part, slots, rows, flag)
     assert flag.item() == 0, "flag raised for sums inside (1e-30, 1e30)"
-    # fp32 sum of <= 70 positive terms: < 70 * 2^-24 = 4.2e-6, plus the rounding of 1 / s: 1e-5.  Every slot holds
-    # >= 1 / (3 * slots) of its row's sum, so a dropped slot or a read spare slot (NaN) is far outside.
+    # fp32 sum of positive terms, <= 32 per lane (1014 slots) then a 5-level shuffle tree: < 37 * 2^-24 = 2.2e-6, plus
+    # the rounding of 1 / s: 1e-5.  Every slot holds >= 1 / (3 * slots) of its row's sum (>= 3.3e-4 at 1014 slots), so a
+    # dropped slot or a read spare slot (NaN) is far outside.
     rel = (base.double() - want).abs() / want
     assert torch.isfinite(rel).all() and rel.max().item() <= 1e-5, f"rowscale: max rel err {rel.max().item():.3e}"
     flag = _flag(1)
@@ -177,7 +182,7 @@ def test_pexp_stat_combine_rowscale_and_flag(svr2lib, slots):
             assert torch.equal(rs[others], base[others]), "a flagged row changed the other rows' rowscale"
 
 
-@pytest.mark.parametrize("slots,rows", [(1, 1), (5, 3), (33, 203), (70, 203)])
+@pytest.mark.parametrize("slots,rows", [(1, 1), (5, 3), (33, 203), (70, 203), (64, 8448), (64, 2880)])   # 64: 4K sampled keys
 def test_rowstat_max_reference_exponent_and_flag_reset(svr2lib, slots, rows):
     """mhat[row] = max over the slots' .x (exact), -inf slots included; the spare slot past `slots` holds +1e9 and every
     .y is NaN (neither is read).  The flag is cleared for any row count, and a NULL flag_reset is accepted."""
@@ -200,7 +205,8 @@ def test_rowstat_max_reference_exponent_and_flag_reset(svr2lib, slots, rows):
             assert flag.item() == 0, f"rowstat_max did not clear the flag (rows = {rows})"
 
 
-@pytest.mark.parametrize("slots,rows", [(1, 5), (6, 203), (33, 203), (70, 203)])
+@pytest.mark.parametrize("slots,rows", [(1, 5), (6, 203), (33, 203), (70, 203), (254, 2880), (254, 8448), (1014, 2880),
+                                        (1014, 8448)])
 def test_rowstat_combine_lse(svr2lib, slots, rows):
     """lse[row] = max + log2(sum_i l_i 2^(m_i - max)) against fp64, with -inf slots (the empty half-tiles of a ragged N;
     their .y is NaN and must not be read), a spare slot past `slots` that would dominate if read, and a row whose
@@ -224,8 +230,9 @@ def test_rowstat_combine_lse(svr2lib, slots, rows):
     svr2lib.call("svr2_rowstat_combine", svr2lib.ptr(part), slots, ld, svr2lib.ptr(lse), rows, svr2lib.stream())
     torch.cuda.synchronize()
     assert lse[rows - 1].item() == -INF, f"all -inf slots: lse = {lse[rows - 1].item()}"
-    # |lse| < 48: fp32 ulp <= 3.8e-6, exp2f / log2f and the fp32 sum of <= 70 terms add < 8e-6: 2e-5.  Every finite
-    # slot carries >= 2^-3 / (2 * 70) of its row's sum, so a dropped or extra slot moves lse by > 1e-3.
+    # |lse| < 48: fp32 ulp <= 3.8e-6, exp2f / log2f and the fp32 sum (<= 32 terms per lane, a 5-level tree) add < 8e-6:
+    # 2e-5.  Every finite slot carries >= 2^-3 / (2 * slots) of its row's sum, so a dropped or extra slot moves lse by
+    # > 1e-3 at 70 slots, > 8e-5 at 1014.
     err = (lse[:rows - 1].double() - want[:rows - 1]).abs()
     assert torch.isfinite(err).all() and err.max().item() <= 2e-5, f"lse: max abs err {err.max().item():.3e}"
 

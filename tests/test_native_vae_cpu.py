@@ -25,6 +25,7 @@ def cpu_vae():
 
 @pytest.mark.parametrize("direction,T,H,W,split", [
     ("dec", 3, 6, 10, None), ("dec", 5, 6, 10, 8), ("dec", 6, 5, 7, 4), ("dec", 1, 40, 24, None),
+    ("dec", 1, 270, 480, None),         # the 4K latent: mid-block attention at n = 129 600 in 16 query chunks
     ("enc", 9, 48, 80, None), ("enc", 17, 48, 80, 8), ("enc", 13, 32, 48, 4), ("enc", 6, 32, 48, 4), ("enc", 1, 128, 160, None),
 ])
 def test_native_vae_sequence_matches_python(cpu_vae, tracer, tmp_path, direction, T, H, W, split):
